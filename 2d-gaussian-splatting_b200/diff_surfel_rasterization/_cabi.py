@@ -101,16 +101,26 @@ def load():
             f"{LIB_PATH} not found: build the sm_90a CUDA library first "
             "(python 2d-gaussian-splatting_b200/build.py, or __graft_entry__.build()). "
             "diff_surfel_rasterization has no CPU fallback.")
-    lib = ctypes.CDLL(LIB_PATH)
+    _lib = load_handle(LIB_PATH)
+    return _lib
+
+
+def load_handle(path):
+    """Open a build of the library at `path` (the main one, or a test variant under lib/variants/) as a separate
+    handle with every signature of SIGNATURES configured on it; the global handle of load() is left alone."""
+    if not os.path.exists(path):
+        raise ImportError(f"{path} not found: build it first (python 2d-gaussian-splatting_b200/build.py)")
+    lib = ctypes.CDLL(path)
     for name, (res, args) in SIGNATURES.items():
         fn = getattr(lib, name)          # AttributeError if the symbol is not exported
         fn.restype, fn.argtypes = res, args
     if lib.surfel_abi_version() != 3:
-        raise ImportError("libsurfel_b200.so ABI version mismatch")
-    _lib = lib
+        raise ImportError(f"{path}: ABI version mismatch")
     return lib
 
 
-def check(status):
+def check(status, lib=None):
+    """Raise on a non-zero status, with the error string of the library handle that returned it (default: the
+    global one)."""
     if status != 0:
-        raise RuntimeError("surfel rasterizer: " + load().surfel_last_error().decode())
+        raise RuntimeError("surfel rasterizer: " + (lib or load()).surfel_last_error().decode())

@@ -125,20 +125,45 @@ def render_fwd(pre, binned, bg, W, H, f64=False):
     return out
 
 
+ABS_LAYOUT = (("dL_dtransMat", 0, 9), ("dL_dmean2D", 9, 11), ("dL_dopacity", 11, 12), ("dL_dnormal", 12, 15),
+              ("dL_dcolors", 15, 18))
+
+
 def render_bwd(pre, binned, img, bg, dL_dcolor, dL_dothers, W, H, lowpass_quirk=True, f64=False):
-    """A.4.  f64=True: the per-pair arithmetic in double (yardstick for float32 rounding noise, not a parity target)."""
+    """A.4.  f64=True: the per-pair arithmetic in double (yardstick for float32 rounding noise, not a parity target).
+    With f64=True the result also holds out["abs"][key]: per entry, the sum of the absolute per-pair contributions."""
     P = pre["radii"].shape[0]
     out = dict(dL_dtransMat=np.zeros((P, 9), np.float64), dL_dmean2D=np.zeros((P, 2), np.float64),
                dL_dopacity=np.zeros(P, np.float64), dL_dnormal=np.zeros((P, 3), np.float64),
                dL_dcolors=np.zeros((P, 3), np.float64))
-    fn = lib().oracle_render_bwd_f64 if f64 else lib().oracle_render_bwd
-    fn(W, H, _p(binned["ranges"]), _p(binned["vals_sorted"]), _p(pre["xy"]),
-                            _p(pre["transMat"]), _p(pre["normal_opacity"]), _p(pre["rgb"]),
-                            _p(_f32(bg)), _p(img["accum"]), _p(img["n_contrib"]),
-                            _p(_f32(dL_dcolor)), _p(_f32(dL_dothers)), int(bool(lowpass_quirk)),
-                            _p(out["dL_dtransMat"]), _p(out["dL_dmean2D"]), _p(out["dL_dopacity"]),
-                            _p(out["dL_dnormal"]), _p(out["dL_dcolors"]))
+    args = [W, H, _p(binned["ranges"]), _p(binned["vals_sorted"]), _p(pre["xy"]),
+            _p(pre["transMat"]), _p(pre["normal_opacity"]), _p(pre["rgb"]),
+            _p(_f32(bg)), _p(img["accum"]), _p(img["n_contrib"]),
+            _p(_f32(dL_dcolor)), _p(_f32(dL_dothers)), int(bool(lowpass_quirk)),
+            _p(out["dL_dtransMat"]), _p(out["dL_dmean2D"]), _p(out["dL_dopacity"]),
+            _p(out["dL_dnormal"]), _p(out["dL_dcolors"])]
+    if f64:
+        absum = np.zeros((P, 18), np.float64)
+        lib().oracle_render_bwd_f64(*args, _p(absum))
+        out["abs"] = {k: absum[:, a:b].reshape(out[k].shape) for k, a, b in ABS_LAYOUT}
+    else:
+        lib().oracle_render_bwd(*args)
     return out
+
+
+MARGIN_NAMES = ("alpha_min", "alpha_clamp", "rho_branch", "near", "t_min", "median", "pz", "power")
+
+
+def decision_margins(pre, binned, W, H, slack=1e-3):
+    """Per-pixel smallest relative distance of any evaluated (pixel, splat) pair to each discontinuity of A.3, in
+    float64 (oracle_decision_margins).  Returns (dict name -> (H, W) array, per-splat smallest margin (P,))."""
+    P = pre["radii"].shape[0]
+    m = np.zeros((len(MARGIN_NAMES), H, W), np.float64)
+    per_splat = np.zeros(P, np.float64)
+    lib().oracle_decision_margins(W, H, P, _p(binned["ranges"]), _p(binned["vals_sorted"]), _p(pre["xy"]),
+                                  _p(pre["transMat"]), _p(pre["normal_opacity"]), ctypes.c_double(slack),
+                                  _p(m), _p(per_splat))
+    return dict(zip(MARGIN_NAMES, m)), per_splat
 
 
 def preprocess_bwd(means3D, scales, rotations, shs, pre, rb, viewmatrix, projmatrix, campos, W, H,

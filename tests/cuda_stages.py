@@ -17,9 +17,10 @@ def _p(t):
 
 
 class CudaPipeline:
-    def __init__(self, scene, cam, bg, sh_degree=3, scale_modifier=1.0, tile_rows=(0, 0), fused_count=True):
+    def __init__(self, scene, cam, bg, sh_degree=3, scale_modifier=1.0, tile_rows=(0, 0), fused_count=True, lib=None):
+        """lib: a library handle from _cabi.load_handle() (a test variant of the kernels); default the main library."""
         self.fused_count = fused_count
-        self.lib = _cabi.load()
+        self.lib = _cabi.load() if lib is None else lib
         self.W, self.H = cam["W"], cam["H"]
         self.gx, self.gy = (self.W + 15) // 16, (self.H + 15) // 16
         g = lambda k: scene.get(k)
@@ -34,6 +35,9 @@ class CudaPipeline:
                                        self.bg.data_ptr(), self.vm.data_ptr(), self.pm.data_ptr(), self.campos.data_ptr())
         self.stream = torch.cuda.current_stream().cuda_stream
 
+    def _check(self, status):
+        _cabi.check(status, self.lib)
+
     # ---- stage 1 ----
     def preprocess(self):
         lib, P = self.lib, self.P
@@ -43,7 +47,7 @@ class CudaPipeline:
         self.geom = torch.full((lib.surfel_geom_bytes(P),), 0xFF, dtype=torch.uint8, device="cuda")
         self.img = torch.full((lib.surfel_image_bytes(self.W, self.H),), 0xFF, dtype=torch.uint8, device="cuda")
         host_R = torch.zeros(1, dtype=torch.int32).pin_memory()
-        _cabi.check(lib.surfel_forward_preprocess(
+        self._check(lib.surfel_forward_preprocess(
             ctypes.byref(self.cs), P, self.M, _p(self.means3D), _p(self.opacities), _p(self.scales),
             _p(self.rotations), _p(self.transMat_precomp), _p(self.shs), _p(self.colors_precomp),
             self.radii.data_ptr(), self.geom.data_ptr(), self.img.data_ptr() if self.fused_count else None,
@@ -76,7 +80,7 @@ class CudaPipeline:
     def duplicate(self):
         lib = self.lib
         self.binning = torch.full((lib.surfel_binning_bytes(self.R, self.W, self.H),), 0xFF, dtype=torch.uint8, device="cuda")
-        _cabi.check(lib.surfel_bin_duplicate(ctypes.byref(self.cs), self.P, self.R, self.geom.data_ptr(),
+        self._check(lib.surfel_bin_duplicate(ctypes.byref(self.cs), self.P, self.R, self.geom.data_ptr(),
                                              self.radii.data_ptr(), self.binning.data_ptr(), self.stream))
         torch.cuda.synchronize()
         o = self._bin_views()
@@ -89,7 +93,7 @@ class CudaPipeline:
         """Production binning path (tile buckets + per-tile sort); same outputs as duplicate()+sort()."""
         lib = self.lib
         self.binning = torch.full((lib.surfel_binning_bytes(self.R, self.W, self.H),), 0xFF, dtype=torch.uint8, device="cuda")
-        _cabi.check(lib.surfel_bin_bucket(ctypes.byref(self.cs), self.P, self.R, self.geom.data_ptr(),
+        self._check(lib.surfel_bin_bucket(ctypes.byref(self.cs), self.P, self.R, self.geom.data_ptr(),
                                           self.radii.data_ptr(), self.binning.data_ptr(),
                                           self.img.data_ptr() if self.fused_count else None, 1, self.stream))
         torch.cuda.synchronize()
@@ -101,7 +105,7 @@ class CudaPipeline:
                     ranges=b[o[4]:o[4] + 8 * tiles].view(np.uint32).reshape(tiles, 2).copy())
 
     def sort(self):
-        _cabi.check(self.lib.surfel_bin_sort(ctypes.byref(self.cs), self.R, self.binning.data_ptr(), self.stream))
+        self._check(self.lib.surfel_bin_sort(ctypes.byref(self.cs), self.R, self.binning.data_ptr(), self.stream))
         torch.cuda.synchronize()
         o = self._bin_views()
         b = self.binning.cpu().numpy()
@@ -115,7 +119,7 @@ class CudaPipeline:
         band = self.cs.tile_row_begin != 0 or self.cs.tile_row_end != 0      # a band leaves the other rows untouched
         fill = 0.0 if band else float("nan")
         self.color = torch.full((3, H, W), fill, device="cuda"); self.others = torch.full((7, H, W), fill, device="cuda")
-        _cabi.check(lib.surfel_render_forward(ctypes.byref(self.cs), self.R, self.geom.data_ptr(),
+        self._check(lib.surfel_render_forward(ctypes.byref(self.cs), self.R, self.geom.data_ptr(),
                                               self.binning.data_ptr(), self.img.data_ptr(),
                                               self.color.data_ptr(), self.others.data_ptr(), self.stream))
         torch.cuda.synchronize()
@@ -138,7 +142,7 @@ class CudaPipeline:
         scratch = e(max(P, 1), lib.surfel_grad_scratch_floats())
         out = dict(dL_dmeans2D=e(P, 3), dL_dcolors=e(P, 3), dL_dopacity=e(P, 1), dL_dmeans3D=e(P, 3),
                    dL_dtransMat=e(P, 9), dL_dshs=e(P, max(M, 1), 3), dL_dscales=e(P, 2), dL_drotations=e(P, 4))
-        _cabi.check(lib.surfel_backward(
+        self._check(lib.surfel_backward(
             ctypes.byref(self.cs), P, M, self.R, _p(self.means3D), _p(self.scales), _p(self.rotations),
             _p(self.transMat_precomp), _p(self.shs), int(self.colors_precomp is not None),
             self.radii.data_ptr(), self.geom.data_ptr(), self.binning.data_ptr(), self.img.data_ptr(),
@@ -150,7 +154,7 @@ class CudaPipeline:
             int(lowpass_quirk), self.stream))
         self.cs.sh_grad_deferred = 0
         if defer_sh and M:
-            _cabi.check(lib.surfel_sh_grad_expand(P, M, int(self.cs.sh_degree), self.means3D.data_ptr(), self.campos.data_ptr(),
+            self._check(lib.surfel_sh_grad_expand(P, M, int(self.cs.sh_degree), self.means3D.data_ptr(), self.campos.data_ptr(),
                                                   out["dL_dcolors"].data_ptr(), out["dL_dshs"].data_ptr(), self.stream))
         torch.cuda.synchronize()
         res = {k: v.cpu().numpy() for k, v in out.items()}
