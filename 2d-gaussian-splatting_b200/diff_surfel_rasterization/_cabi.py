@@ -69,6 +69,8 @@ SIGNATURES = {
     "surfel_densify_stats": (c_int, [c_int] + [c_void_p] * 5 + [c_void_p]),
     "surfel_ply_unpack": (c_int, [c_int, c_int, c_void_p, ctypes.POINTER(ctypes.c_int32), c_int] + [c_void_p] * 5 + [c_void_p]),
     "surfel_ply_pack": (c_int, [c_int] + [c_void_p] * 7 + [c_void_p]),
+    "surfel_knn_workspace_bytes": (c_size_t, [c_int]),
+    "surfel_knn_mean_sq_dist": (c_int, [c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "surfel_launch_count": (ctypes.c_ulonglong, []),
     "surfel_profile_enable": (None, [c_int]),
     "surfel_profile_num_stages": (c_int, []),

@@ -262,6 +262,18 @@ int surfel_ply_unpack(int P, int row_floats, const float* rows, const int32_t* c
 int surfel_ply_pack(int P, const float* xyz, const float* features_dc, const float* features_rest,
                     const float* opacity, const float* scaling, const float* rotation, float* rows, void* stream);
 
+/* ---- Model initialisation: simple_knn.distCUDA2 of /root/reference/scene/gaussian_model.py:20, :134 ----
+ * out[i] = mean of the squared distances from point i to its three nearest OTHER points (rules: DESIGN.md
+ * §7g, csrc/knn.cu).  Exact; d2 = (dx*dx + dy*dy) + dz*dz in float32 without FMA, result ((a+b)+c)/3.0f
+ * over the three smallest, so it is bit-reproducible.  Fewer than three finite other points: the mean over
+ * those that exist (0 if none).  A row with a NaN / inf coordinate is nobody's neighbour and gets NaN.
+ * xyz: (P,3) contiguous float32; out: (P) float32; workspace: surfel_knn_workspace_bytes(P) bytes
+ * (uninitialised is fine), its size passed as workspace_bytes.  P = 0 launches nothing; P must be below
+ * 2^30 (surfel_knn_workspace_bytes returns 0 for a P out of range). */
+size_t surfel_knn_workspace_bytes(int P);
+int surfel_knn_mean_sq_dist(int P, const float* xyz, float* out, void* workspace, size_t workspace_bytes,
+                            void* stream);
+
 /* Instrumentation used by bench.py: number of kernels this library has launched in this process,
  * and optional per-stage CUDA-event timing (events recorded on the launching stream around each
  * kernel while enabled; surfel_profile_read() waits for them and returns summed ms / launch counts
