@@ -37,6 +37,17 @@ class AdamGroup(ctypes.Structure):
 
 ADAM_MAX_GROUPS = 8
 
+
+class DensifyGroup(ctypes.Structure):
+    """struct surfel_densify_group (include/surfel_rasterizer.h)."""
+    _fields_ = [("param", c_void_p), ("exp_avg", c_void_p), ("exp_avg_sq", c_void_p),
+                ("out_param", c_void_p), ("out_exp_avg", c_void_p), ("out_exp_avg_sq", c_void_p),
+                ("row_floats", c_int), ("kind", c_int)]
+
+
+DENSIFY_MAX_GROUPS = 8
+DENSIFY_COPY, DENSIFY_XYZ, DENSIFY_SCALING, DENSIFY_ROTATION = 0, 1, 2, 3
+
 # name -> (restype, argtypes); every symbol include/surfel_rasterizer.h declares
 SIGNATURES = {
     "surfel_abi_version": (c_int, []),
@@ -71,6 +82,11 @@ SIGNATURES = {
     "surfel_ply_pack": (c_int, [c_int] + [c_void_p] * 7 + [c_void_p]),
     "surfel_knn_workspace_bytes": (c_size_t, [c_int]),
     "surfel_knn_mean_sq_dist": (c_int, [c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "surfel_densify_workspace_bytes": (c_size_t, [c_int]),
+    "surfel_densify_plan": (c_int, [c_int] + [c_void_p] * 4 + [ctypes.c_double] * 4 + [c_int, ctypes.c_double]
+                            + [c_void_p, c_size_t, c_void_p, c_void_p]),
+    "surfel_densify_apply": (c_int, [c_int, c_int, c_int, c_int, ctypes.POINTER(DensifyGroup), c_void_p, c_void_p,
+                                     c_size_t, c_void_p]),
     "surfel_launch_count": (ctypes.c_ulonglong, []),
     "surfel_profile_enable": (None, [c_int]),
     "surfel_profile_num_stages": (c_int, []),

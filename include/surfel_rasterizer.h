@@ -274,6 +274,45 @@ size_t surfel_knn_workspace_bytes(int P);
 int surfel_knn_mean_sq_dist(int P, const float* xyz, float* out, void* workspace, size_t workspace_bytes,
                             void* stream);
 
+/* ---- Densification: GaussianModel.densify_and_prune of the reference trainer ----------------------
+ * (scene/gaussian_model.py:348-403, train.py:132; rules in DESIGN.md §7h, csrc/densify.cu).  Clone, split
+ * and the final prune of every parameter group and its Adam moments, as one compaction:
+ *  surfel_densify_plan decides every row from (xyz_gradient_accum (P,1), denom (P,1), scaling (P,2),
+ *   opacity (P,1)) and writes totals[4] (device int32) = { kept originals, kept clones, split rows S, P' }.
+ *   The thresholds are the doubles Python forms (max_grad, min_opacity, percent_dense * extent,
+ *   0.1 * extent, max_screen_size), each rounded once to float32 as torch does when it compares; the
+ *   screen-size and world-size prune apply only when use_max_screen_size is non-zero.
+ *  surfel_densify_apply then writes the P' output rows of every group: kept originals (moments kept) |
+ *   kept clones | kept split copies A | kept split copies B (zero moments).  P_out and n_split are
+ *   totals[3] and totals[2] as read back by the caller; z is the (2 n_split, 3) standard normal draw (rows
+ *   [0, S) for copies A, [S, 2S) for copies B, in split-row order).  A group with NULL moments has no
+ *   optimizer state and is gathered without it.  At most one group each of kind XYZ (3 floats per row),
+ *   SCALING (2) and ROTATION (4), and a table with the XYZ group needs the other two (split copies' xyz reads
+ *   them); the others are COPY.  The groups of one plan may be split over several apply calls (the Python
+ *   wrapper applies f_rest first and frees its old tensors before it allocates the other groups' new ones).
+ * All float arrays are contiguous float32; the workspace is surfel_densify_workspace_bytes(P) bytes
+ * (uninitialised is fine) and must be the same between the plan and the apply of one call.  P must be
+ * below 2^30 (surfel_densify_workspace_bytes returns 0 for a P out of range). */
+#define SURFEL_DENSIFY_MAX_GROUPS 8
+enum { SURFEL_DENSIFY_COPY = 0, SURFEL_DENSIFY_XYZ = 1, SURFEL_DENSIFY_SCALING = 2, SURFEL_DENSIFY_ROTATION = 3 };
+typedef struct surfel_densify_group {
+    const float* param;        /* P rows of row_floats */
+    const float* exp_avg;      /* P rows, or NULL (no state) */
+    const float* exp_avg_sq;   /* P rows, or NULL (no state) */
+    float* out_param;          /* P' rows */
+    float* out_exp_avg;        /* P' rows; NULL iff exp_avg is NULL */
+    float* out_exp_avg_sq;     /* P' rows; NULL iff exp_avg_sq is NULL */
+    int row_floats;
+    int kind;                  /* SURFEL_DENSIFY_* */
+} surfel_densify_group_t;
+size_t surfel_densify_workspace_bytes(int P);
+int surfel_densify_plan(int P, const float* xyz_gradient_accum, const float* denom, const float* scaling,
+                        const float* opacity, double max_grad, double min_opacity, double clone_max_scale,
+                        double prune_max_scale, int use_max_screen_size, double max_screen_size, void* workspace,
+                        size_t workspace_bytes, int32_t* totals, void* stream);
+int surfel_densify_apply(int P, int P_out, int n_split, int n_groups, const surfel_densify_group_t* groups,
+                         const float* z, const void* workspace, size_t workspace_bytes, void* stream);
+
 /* Instrumentation used by bench.py: number of kernels this library has launched in this process,
  * and optional per-stage CUDA-event timing (events recorded on the launching stream around each
  * kernel while enabled; surfel_profile_read() waits for them and returns summed ms / launch counts
