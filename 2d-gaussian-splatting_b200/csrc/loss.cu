@@ -132,11 +132,19 @@ l1_ssim_bwd_kernel(int C, int H, int W, const float* __restrict__ img, const flo
 
 using namespace surfel;
 
+// one block per 16x16 tile per channel: grid y and z are limited to 65535
+static bool loss_shape_ok(int C, int H, int W) {
+    return C > 0 && H > 0 && W > 0 && C <= 65535 && (H + kLT - 1) / kLT <= 65535;
+}
+
 extern "C" {
 
 int surfel_l1_ssim_forward(int C, int H, int W, const float* img, const float* gt, float* dmu1,
                            float* ds11, float* ds12, double* sums2, void* stream) {
-    if (C <= 0 || H <= 0 || W <= 0) { surfel_set_error("surfel_l1_ssim_forward: bad shape"); return 1; }
+    if (!loss_shape_ok(C, H, W)) { surfel_set_error("surfel_l1_ssim_forward: bad shape"); return 1; }
+    if (!img || !gt || !dmu1 || !ds11 || !ds12 || !sums2) {
+        surfel_set_error("surfel_l1_ssim_forward: NULL required pointer"); return 1;
+    }
     cudaStream_t st = (cudaStream_t)stream;
     static bool init[kMaxDevices] = {};                 // the window lives in __constant__ memory: one copy per device
     const int slot = current_device_slot();
@@ -159,7 +167,10 @@ int surfel_l1_ssim_forward(int C, int H, int W, const float* img, const float* g
 int surfel_l1_ssim_backward(int C, int H, int W, const float* img, const float* gt, const float* dmu1,
                             const float* ds11, const float* ds12, const float* gscale2, float* g_img,
                             void* stream) {
-    if (C <= 0 || H <= 0 || W <= 0) { surfel_set_error("surfel_l1_ssim_backward: bad shape"); return 1; }
+    if (!loss_shape_ok(C, H, W)) { surfel_set_error("surfel_l1_ssim_backward: bad shape"); return 1; }
+    if (!img || !gt || !dmu1 || !ds11 || !ds12 || !gscale2 || !g_img) {
+        surfel_set_error("surfel_l1_ssim_backward: NULL required pointer"); return 1;
+    }
     dim3 grid((W + kLT - 1) / kLT, (H + kLT - 1) / kLT, C), blk(kLT, kLT);
     prof_count_launch();
     l1_ssim_bwd_kernel<<<grid, blk, 0, (cudaStream_t)stream>>>(C, H, W, img, gt, dmu1, ds11, ds12, gscale2, g_img);

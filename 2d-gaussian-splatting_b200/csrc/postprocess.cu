@@ -128,9 +128,12 @@ __global__ void post_bwd_allmap_kernel(int W, int H, float ratio, const float* _
     const float gd = dP[0] * r0 + dP[1] * r1 + dP[2] * r2 + (g_surf_depth ? g_surf_depth[i] : 0.0f);
     const float D = allmap[i], A = allmap[N + i], med = allmap[5 * N + i];
     const float ex = D / A;
-    const float g_ex = is_finite(ex) ? gd * (1.0f - ratio) : 0.0f;
-    g_allmap[i] = g_ex / A;
-    g_allmap[N + i] = -g_ex * D / (A * A);
+    // nan_to_num passes no gradient where D/alpha is not finite (a hole, alpha == 0); there the chain rule's
+    // 0 / alpha would be 0/0, so the fused backward writes 0 where the reference's autograd yields NaN
+    const bool fin = is_finite(ex);
+    const float g_ex = fin ? gd * (1.0f - ratio) : 0.0f;
+    g_allmap[i] = fin ? g_ex / A : 0.0f;
+    g_allmap[N + i] = fin ? -g_ex * D / (A * A) : 0.0f;
     g_allmap[5 * N + i] = is_finite(med) ? gd * ratio : 0.0f;
     g_allmap[6 * N + i] = 0.0f;
     float gn[3] = {0, 0, 0};
@@ -143,12 +146,20 @@ __global__ void post_bwd_allmap_kernel(int W, int H, float ratio, const float* _
 
 using namespace surfel;
 
+// the kernels index the 7 planes of allmap with int, and the 32x8 grid's y extent is limited to 65535
+static bool post_size_ok(int W, int H) {
+    return W > 0 && H > 0 && 7LL * W * H <= 0x7fffffffLL && (H + 7) / 8 <= 65535;
+}
+
 extern "C" {
 
 int surfel_post_forward(int W, int H, float depth_ratio, const float* allmap, const float* rot,
                         const float* rays, float* rend_normal, float* surf_depth, float* surf_normal,
                         void* stream) {
-    if (W <= 0 || H <= 0) { surfel_set_error("surfel_post_forward: bad size"); return 1; }
+    if (!post_size_ok(W, H)) { surfel_set_error("surfel_post_forward: bad size"); return 1; }
+    if (!allmap || !rot || !rays || !rend_normal || !surf_depth || !surf_normal) {
+        surfel_set_error("surfel_post_forward: NULL required pointer"); return 1;
+    }
     cudaStream_t st = (cudaStream_t)stream;
     const int N = W * H;
     prof_count_launch(); prof_count_launch();
@@ -164,7 +175,10 @@ int surfel_post_backward(int W, int H, float depth_ratio, const float* allmap, c
                          const float* rays, const float* surf_depth, const float* g_rend_normal,
                          const float* g_surf_depth, const float* g_surf_normal, float* tmp6,
                          float* g_allmap, void* stream) {
-    if (W <= 0 || H <= 0) { surfel_set_error("surfel_post_backward: bad size"); return 1; }
+    if (!post_size_ok(W, H)) { surfel_set_error("surfel_post_backward: bad size"); return 1; }
+    if (!allmap || !rot || !rays || !surf_depth || !tmp6 || !g_allmap) {
+        surfel_set_error("surfel_post_backward: NULL required pointer"); return 1;
+    }
     cudaStream_t st = (cudaStream_t)stream;
     dim3 blk(32, 8), grd((W + 31) / 32, (H + 7) / 8);
     prof_count_launch(); prof_count_launch();

@@ -71,6 +71,14 @@ class _SurfaceOutputs(torch.autograd.Function):
 def surface_outputs(allmap, viewpoint_camera, depth_ratio):
     """allmap (7,H,W) from GaussianRasterizer -> dict with the reference's keys."""
     W, H = int(viewpoint_camera.image_width), int(viewpoint_camera.image_height)
+    if not torch.is_tensor(allmap) or not allmap.is_cuda:
+        raise RuntimeError("surface_outputs: allmap must be a CUDA tensor (no CPU path)")
+    if tuple(allmap.shape) != (7, H, W):
+        raise RuntimeError(f"surface_outputs: allmap must be (7, {H}, {W}) for this camera, got {tuple(allmap.shape)}")
+    for name in ("world_view_transform", "full_proj_transform"):
+        m = getattr(viewpoint_camera, name)
+        if not torch.is_tensor(m) or m.device != allmap.device or tuple(m.shape) != (4, 4):
+            raise RuntimeError(f"surface_outputs: camera {name} must be a (4, 4) tensor on {allmap.device}")
     rot, rays = _view_matrices(viewpoint_camera.world_view_transform, viewpoint_camera.full_proj_transform, W, H)
     rend_normal, surf_depth, surf_normal = _SurfaceOutputs.apply(allmap, rot, rays, depth_ratio)
     return {"rend_alpha": allmap[1:2], "rend_normal": rend_normal, "rend_dist": allmap[6:7],

@@ -1,10 +1,17 @@
-"""Fused L1+SSIM loss (SURVEY §8f row f2) against a PyTorch restatement of the reference's
-l1_loss / ssim (/root/reference/utils/loss_utils.py:6-7, :43-73; combined at train.py:73-74)."""
+"""Fused L1+SSIM loss (SURVEY §8f row f2) held, entry by entry and with no budget, to the float64
+evaluation of the reference's l1_loss / ssim (/root/reference/utils/loss_utils.py:6-7, :43-73; combined at
+train.py:73-74) in tests/tail_loss_exact.py, and replayed against the reference's own stored values and
+gradients.  reference_loss is the PyTorch restatement the golden CPU test pins to the reference."""
 from math import exp
 
+import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
+
+import tail_loss_exact as X
+import tail_loss_scenes as TS
+from parity_bars import record_stats
 
 pytestmark = pytest.mark.gpu
 
@@ -12,8 +19,9 @@ pytestmark = pytest.mark.gpu
 def reference_loss(img, gt, lam):
     g = torch.tensor([exp(-(x - 5) ** 2 / float(2 * 1.5 ** 2)) for x in range(11)])
     g = (g / g.sum()).unsqueeze(1)
-    window = g.mm(g.t()).float().unsqueeze(0).unsqueeze(0).expand(3, 1, 11, 11).contiguous().to(img.device)
-    conv = lambda t: F.conv2d(t, window, padding=5, groups=3)
+    C = img.size(-3)
+    window = g.mm(g.t()).float().unsqueeze(0).unsqueeze(0).expand(C, 1, 11, 11).contiguous().to(img)
+    conv = lambda t: F.conv2d(t, window, padding=5, groups=C)
     mu1, mu2 = conv(img), conv(gt)
     s1, s2, s12 = conv(img * img) - mu1.pow(2), conv(gt * gt) - mu2.pow(2), conv(img * gt) - mu1 * mu2
     C1, C2 = 0.01 ** 2, 0.03 ** 2
@@ -21,20 +29,111 @@ def reference_loss(img, gt, lam):
     return (1.0 - lam) * torch.abs(img - gt).mean() + lam * (1.0 - ssim)
 
 
-@pytest.mark.parametrize("shape,lam", [((3, 97, 131), 0.2), ((3, 256, 320), 0.2), ((3, 64, 48), 1.0), ((3, 33, 17), 0.0)])
-def test_fused_l1_ssim_matches_reference(cuda_lib, shape, lam):
+
+# Tolerances: |fused - exact| <= TOL * bound for the value and for every gradient entry (bounds of
+# tail_loss_exact.loss_f64, in which a float32 emulation of the kernel reaches 0.12 and 0.03).  Cut at about 4x
+# the worst value observed on an H100 80GB HBM3 (700 W power limit) over every case below.
+VALUE_TOL = 0.32        # worst observed 0.080 (3x33x17, lambda 0)
+GRAD_TOL = 0.33         # worst observed 0.082 (3x1x1, lambda 0.2)
+
+
+def _fused(img, gt, lam, gout=1.0):
     from diff_surfel_rasterization.loss import l1_ssim_loss
-    g = torch.Generator("cpu").manual_seed(shape[1])
-    base = torch.rand(*shape, generator=g)
-    gt = (base + 0.1 * torch.randn(*shape, generator=g)).clamp(0, 1).cuda()
-    img0 = (base + 0.15 * torch.randn(*shape, generator=g)).clamp(0, 1).cuda()
-    res = {}
-    for name, fn in (("ref", reference_loss), ("fused", l1_ssim_loss)):
-        img = img0.clone().requires_grad_(True)
-        loss = fn(img, gt, lam)
-        (loss * 3.0).backward()
-        res[name] = (float(loss.detach()), img.grad)
-    assert abs(res["ref"][0] - res["fused"][0]) < 2e-5 * max(1.0, abs(res["ref"][0])), (res["ref"][0], res["fused"][0])
-    gr, gf = res["ref"][1], res["fused"][1]
-    err = (gr - gf).abs().max() / gr.abs().max().clamp_min(1e-12)
-    assert float(err) < 2e-4, float(err)
+    x = img.cuda().requires_grad_(True)
+    loss = l1_ssim_loss(x, gt.cuda(), lam)
+    (loss * gout).backward()
+    return float(loss.detach()), x.grad.double()
+
+
+def _grad_ratio(got, ref, bound):
+    return torch.where(bound > 0, (got - ref).abs() / bound.clamp_min(1e-300),
+                       torch.where(got != ref, torch.inf, 0.0))
+
+
+def test_golden_replay(cuda_lib):
+    """Against the reference's own stored loss values and image gradients (float32): each within its bound
+    of the exact value, so within (TOL + 1) x bound of each other."""
+    g = np.load(X.__file__.replace("tail_loss_exact.py", "golden/ref_tail_loss.npz"))
+    img, gt = torch.from_numpy(g["loss_img"]), torch.from_numpy(g["loss_gt"])
+    for lam in (0.2, 1.0, 0.0):
+        tag = str(lam).replace(".", "p")
+        v, grad = _fused(img, gt, lam)
+        _, _, vb, gb, _, _ = X.loss_f64(img, gt, lam, dev="cuda")
+        assert abs(v - float(g[f"loss_{tag}_value"])) <= (VALUE_TOL + 1) * X.U * vb, lam
+        ref = torch.from_numpy(g[f"loss_{tag}_grad"]).cuda().double()
+        assert float(_grad_ratio(grad, ref, (GRAD_TOL + 1) * X.U * gb).max()) <= 1.0, lam
+
+
+@pytest.mark.parametrize("case", TS.LOSS_CASES, ids=TS.loss_case_id)
+def test_fused_loss_is_exact_within_its_bound(cuda_lib, case):
+    shape, content, lam = case
+    img, gt = TS.image_pair(shape, content)
+    v, grad = _fused(img, gt, lam, gout=3.0)
+    ev, eg, vb, gb, _, _ = X.loss_f64(img, gt, lam, gout=3.0, dev="cuda")
+    assert torch.isfinite(grad).all()
+    rv = abs(v - ev) / (X.U * vb)
+    rg = _grad_ratio(grad, eg, X.U * gb)
+    record_stats(f"loss {TS.loss_case_id(case)} value", np.array([rv]))
+    record_stats(f"loss {TS.loss_case_id(case)} grad", rg.cpu().numpy())
+    assert rv <= VALUE_TOL, rv
+    assert float(rg.max()) <= GRAD_TOL, float(rg.max())
+    if content == "equal":
+        assert v == pytest.approx(0.0, abs=1e-6)
+
+
+def test_batched_input_is_one_loss_over_every_image(cuda_lib):
+    """(2,3,H,W): both images count, the means run over every element and every gradient entry is written,
+    as in the reference's 4-D call."""
+    img, gt = TS.image_pair((2, 3, 40, 56), "noisy")
+    v, grad = _fused(img, gt, 0.2)
+    v0, g0 = _fused(img[0], gt[0], 0.2)
+    v1, g1 = _fused(img[1], gt[1], 0.2)
+    assert v == pytest.approx((v0 + v1) / 2, rel=1e-6)
+    torch.testing.assert_close(grad, torch.stack([g0, g1]) / 2, rtol=1e-5, atol=1e-12)
+    ref = img.clone().requires_grad_(True)
+    reference_loss(ref, gt, 0.2).backward()
+    torch.testing.assert_close(grad.float().cpu(), ref.grad, rtol=1e-3, atol=1e-3 * float(ref.grad.abs().max()))
+
+
+def test_non_contiguous_input_matches_contiguous(cuda_lib):
+    img, gt = TS.image_pair((3, 48, 64), "noisy")
+    v0, g0 = _fused(img, gt, 0.2)
+    img_t = img.transpose(1, 2).contiguous().transpose(1, 2)          # same values, strided
+    gt_t = gt.transpose(1, 2).contiguous().transpose(1, 2)
+    assert not img_t.is_contiguous()
+    v1, g1 = _fused(img_t, gt_t, 0.2)
+    assert v0 == v1 and torch.equal(g0, g1)
+
+
+def test_side_stream_and_second_device(cuda_lib):
+    img, gt = TS.image_pair((3, 97, 131), "noisy")
+    v0, g0 = _fused(img, gt, 0.2)
+    s = torch.cuda.Stream()
+    with torch.cuda.stream(s):
+        from diff_surfel_rasterization.loss import l1_ssim_loss
+        x = img.cuda().requires_grad_(True)
+        loss = l1_ssim_loss(x, gt.cuda(), 0.2)
+        loss.backward()
+    s.synchronize()
+    assert float(loss.detach()) == v0 and torch.equal(x.grad.double(), g0)
+    if torch.cuda.device_count() > 1:                 # the window is uploaded once per device
+        x = img.to("cuda:1").requires_grad_(True)
+        loss = l1_ssim_loss(x, gt.to("cuda:1"), 0.2)
+        loss.backward()
+        assert float(loss.detach()) == v0 and torch.equal(x.grad.double().cuda(0), g0)
+
+
+def test_rejects_bad_inputs_before_launching(cuda_lib):
+    from diff_surfel_rasterization.loss import l1_ssim_loss
+    img, gt = TS.image_pair((3, 20, 24), "noisy")
+    with pytest.raises(RuntimeError, match="image must be a CUDA tensor"):
+        l1_ssim_loss(img, gt.cuda())
+    with pytest.raises(RuntimeError, match="gt must be a CUDA tensor"):
+        l1_ssim_loss(img.cuda(), gt)
+    with pytest.raises(RuntimeError, match="gt shape"):
+        l1_ssim_loss(img.cuda(), gt[:, :10].cuda())
+    with pytest.raises(RuntimeError, match="non-empty"):
+        l1_ssim_loss(img[0].cuda(), gt[0].cuda())
+    if torch.cuda.device_count() > 1:
+        with pytest.raises(RuntimeError, match="gt must be a CUDA tensor"):
+            l1_ssim_loss(img.cuda(), gt.to("cuda:1"))
