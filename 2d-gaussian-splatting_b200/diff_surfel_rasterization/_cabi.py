@@ -48,6 +48,13 @@ class DensifyGroup(ctypes.Structure):
 DENSIFY_MAX_GROUPS = 8
 DENSIFY_COPY, DENSIFY_XYZ, DENSIFY_SCALING, DENSIFY_ROTATION = 0, 1, 2, 3
 
+
+class TsdfFrame(ctypes.Structure):
+    """struct surfel_tsdf_frame (include/surfel_rasterizer.h)."""
+    _fields_ = [("full_proj_transform", c_float * 16), ("height", ctypes.c_int32), ("width", ctypes.c_int32),
+                ("offset", ctypes.c_int64)]
+
+
 # name -> (restype, argtypes); every symbol include/surfel_rasterizer.h declares
 SIGNATURES = {
     "surfel_abi_version": (c_int, []),
@@ -87,6 +94,9 @@ SIGNATURES = {
                             + [c_void_p, c_size_t, c_void_p, c_void_p]),
     "surfel_densify_apply": (c_int, [c_int, c_int, c_int, c_int, ctypes.POINTER(DensifyGroup), c_void_p, c_void_p,
                                      c_size_t, c_void_p]),
+    "surfel_tsdf_eval": (c_int, [ctypes.c_longlong, c_void_p, c_int, ctypes.POINTER(TsdfFrame), ctypes.c_longlong,
+                                 c_void_p, c_void_p, ctypes.POINTER(c_float), ctypes.c_double, ctypes.c_double,
+                                 c_void_p, c_void_p]),
     "surfel_launch_count": (ctypes.c_ulonglong, []),
     "surfel_profile_enable": (None, [c_int]),
     "surfel_profile_num_stages": (c_int, []),

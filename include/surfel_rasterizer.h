@@ -313,6 +313,31 @@ int surfel_densify_plan(int P, const float* xyz_gradient_accum, const float* den
 int surfel_densify_apply(int P, int P_out, int n_split, int n_groups, const surfel_densify_group_t* groups,
                          const float* z, const void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- Mesh extraction: the SDF field of GaussianExtractor.extract_mesh_unbounded ------------------
+ * (utils/mesh_utils.py:184-279 of the reference, `render.py --unbounded`; rules and quirks in DESIGN.md §7i,
+ * csrc/tsdf.cu).  Folds every frame, in table order, into each of n_points samples in one pass:
+ *  field mode (rgb == NULL): points are in contracted space.  Each gets the adaptive truncation
+ *   trunc * 1/(2 - min(|y|, 1.9)) where |y| > 1, is uncontracted and unnormalized (x * radius + center), and
+ *   out[i] (n_points floats) is the running TSDF mean, starting at -1 with weight 1.
+ *  colour mode (rgb != NULL): points are world points, the truncation is the scalar, and out (n_points x 3
+ *   floats) is the running mean of the sampled RGB, starting at 0 with weight 1.
+ * A frame counts for a sample when the projected pix = xy / w lies strictly inside (-1, 1)^2, w > 0 and
+ * depth - w > -trunc, with depth (and RGB) sampled as grid_sample(bilinear, border, align_corners=True).
+ * points: (n_points, 3) contiguous float32 on the device.  frames: a HOST table of n_frames entries, copied to
+ * the device in stream order by the call.  depth: the frames' (H, W) maps concatenated, map_pixels floats, frame
+ * f at frames[f].offset; rgb: their (3, H, W) maps concatenated in the same order (frame f at 3 * offset).
+ * center: 3 host floats; radius and trunc are the doubles the caller forms, each rounded once to float32.
+ * Each side of a frame must be in [1, 2^24] and the frame inside map_pixels.  Runs on `stream`, needs no
+ * workspace and does not synchronise; the result is bit-reproducible (fixed, uncontracted float32 arithmetic). */
+typedef struct surfel_tsdf_frame {
+    float full_proj_transform[16];   /* row-major 4x4: the homogeneous point is the row vector [x y z 1] times it */
+    int32_t height, width;
+    int64_t offset;                  /* element offset of the frame's depth map in `depth` */
+} surfel_tsdf_frame_t;
+int surfel_tsdf_eval(long long n_points, const float* points, int n_frames, const surfel_tsdf_frame_t* frames,
+                     long long map_pixels, const float* depth, const float* rgb, const float* center, double radius,
+                     double trunc, float* out, void* stream);
+
 /* Instrumentation used by bench.py: number of kernels this library has launched in this process,
  * and optional per-stage CUDA-event timing (events recorded on the launching stream around each
  * kernel while enabled; surfel_profile_read() waits for them and returns summed ms / launch counts
