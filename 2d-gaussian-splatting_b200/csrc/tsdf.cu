@@ -25,6 +25,7 @@
 
 #include "../../include/surfel_rasterizer.h"
 #include "common.cuh"
+#include "contraction.cuh"
 #include "profile.h"
 
 namespace surfel {
@@ -82,9 +83,29 @@ __device__ __forceinline__ float sample(const float* __restrict__ map, const Tap
     return v;
 }
 
-template <bool kColour>
+// Where a sample's point comes from: a (N,3) buffer, or (grid mode, DESIGN.md §7j) its index in a side^3 crop of
+// three torch.linspace axes laid out as meshgrid(indexing="ij") lays them out, x slowest.
+struct PointBuffer {
+    const float* pts;
+    __device__ __forceinline__ void load(long long i, float& X, float& Y, float& Z) const {
+        X = pts[3 * i]; Y = pts[3 * i + 1]; Z = pts[3 * i + 2];
+    }
+};
+
+struct PointGrid {
+    LinAxis ax[3];
+    int side;
+    __device__ __forceinline__ void load(long long i, float& X, float& Y, float& Z) const {
+        const long long s = side;
+        X = linspace_at(ax[0], (int)(i / (s * s)), side);
+        Y = linspace_at(ax[1], (int)(i / s % s), side);
+        Z = linspace_at(ax[2], (int)(i % s), side);
+    }
+};
+
+template <bool kColour, class Points>
 __global__ void __launch_bounds__(kTsdfThreads)
-tsdf_kernel(long long N, const float* __restrict__ pts, int V, const TsdfFrame* __restrict__ frames,
+tsdf_kernel(long long N, const Points pts, int V, const TsdfFrame* __restrict__ frames,
             const float* __restrict__ depth, const float* __restrict__ rgb, float cx, float cy, float cz, float radius,
             float trunc0, float* __restrict__ out) {
     __shared__ TsdfFrame sf[kTsdfBatch];
@@ -92,20 +113,12 @@ tsdf_kernel(long long N, const float* __restrict__ pts, int V, const TsdfFrame* 
     const bool live = i < N;
     float X = 0.f, Y = 0.f, Z = 0.f, trunc = trunc0;
     if (live) {
-        X = pts[3 * i]; Y = pts[3 * i + 1]; Z = pts[3 * i + 2];
+        pts.load(i, X, Y, Z);
         if (!kColour) {
             // contracted -> world: adaptive truncation, uncontract, unnormalize
-            const float mag = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(X, X), __fmul_rn(Y, Y)), __fmul_rn(Z, Z)));
+            const float mag = contraction_norm(X, Y, Z);
             if (mag > 1.f) trunc = __fmul_rn(trunc0, __frcp_rn(__fsub_rn(2.f, fminf(mag, 1.9f))));
-            if (!(mag < 1.f)) {
-                const float r = __frcp_rn(__fsub_rn(2.f, mag));
-                X = __fmul_rn(r, __fdiv_rn(X, mag));
-                Y = __fmul_rn(r, __fdiv_rn(Y, mag));
-                Z = __fmul_rn(r, __fdiv_rn(Z, mag));
-            }
-            X = __fadd_rn(__fmul_rn(X, radius), cx);
-            Y = __fadd_rn(__fmul_rn(Y, radius), cy);
-            Z = __fadd_rn(__fmul_rn(Z, radius), cz);
+            inv_contraction(mag, X, Y, Z, radius, cx, cy, cz);
         }
     }
     const float neg_trunc = -trunc;
@@ -151,43 +164,38 @@ tsdf_kernel(long long N, const float* __restrict__ pts, int V, const TsdfFrame* 
     }
 }
 
-}  // namespace surfel
-
-using namespace surfel;
-
-extern "C" {
-
-int surfel_tsdf_eval(long long n_points, const float* points, int n_frames, const surfel_tsdf_frame_t* frames,
-                     long long map_pixels, const float* depth, const float* rgb, const float* center, double radius,
-                     double trunc, float* out, void* stream) {
+// The checks, the frame-table upload and the launch of both entry points; `who` names the entry point in errors.
+template <class Points>
+static int tsdf_run(const char* who, long long n_points, const Points& pts, bool have_pts, int n_frames,
+                    const surfel_tsdf_frame_t* frames, long long map_pixels, const float* depth, const float* rgb,
+                    const float* center, double radius, double trunc, float* out, void* stream) {
     if (n_points < 0 || n_frames < 0 || map_pixels < 0) {
-        surfel_set_error("surfel_tsdf_eval: negative count (n_points %lld, n_frames %d, map_pixels %lld)", n_points,
-                         n_frames, map_pixels);
+        surfel_set_error("%s: negative count (n_points %lld, n_frames %d, map_pixels %lld)", who, n_points, n_frames,
+                         map_pixels);
         return 1;
     }
     const long long blocks = (n_points + kTsdfThreads - 1) / kTsdfThreads;
     if (blocks > 0x7fffffffLL) {
-        surfel_set_error("surfel_tsdf_eval: %lld points exceed the grid limit", n_points);
+        surfel_set_error("%s: %lld points exceed the grid limit", who, n_points);
         return 1;
     }
-    if (!center) { surfel_set_error("surfel_tsdf_eval: NULL center"); return 1; }
-    if (n_frames > 0 && !frames) { surfel_set_error("surfel_tsdf_eval: NULL frame table"); return 1; }
+    if (!center) { surfel_set_error("%s: NULL center", who); return 1; }
+    if (n_frames > 0 && !frames) { surfel_set_error("%s: NULL frame table", who); return 1; }
     for (int f = 0; f < n_frames; f++) {
         const surfel_tsdf_frame_t& F = frames[f];
         if (F.height < 1 || F.width < 1 || F.height > kTsdfMaxSide || F.width > kTsdfMaxSide) {
-            surfel_set_error("surfel_tsdf_eval: frame %d is %d x %d (each side must be in [1, 2^24])", f, F.height,
-                             F.width);
+            surfel_set_error("%s: frame %d is %d x %d (each side must be in [1, 2^24])", who, f, F.height, F.width);
             return 1;
         }
         if (F.offset < 0 || F.offset > map_pixels || (long long)F.height * F.width > map_pixels - F.offset) {
-            surfel_set_error("surfel_tsdf_eval: frame %d (offset %lld, %d x %d) lies outside the %lld map pixels", f,
+            surfel_set_error("%s: frame %d (offset %lld, %d x %d) lies outside the %lld map pixels", who, f,
                              (long long)F.offset, F.height, F.width, map_pixels);
             return 1;
         }
     }
     if (n_points == 0) return 0;
-    if (!points || !out) { surfel_set_error("surfel_tsdf_eval: NULL points or output"); return 1; }
-    if (n_frames > 0 && !depth) { surfel_set_error("surfel_tsdf_eval: NULL depth maps"); return 1; }
+    if (!have_pts || !out) { surfel_set_error("%s: NULL points or output", who); return 1; }
+    if (n_frames > 0 && !depth) { surfel_set_error("%s: NULL depth maps", who); return 1; }
 
     cudaStream_t st = (cudaStream_t)stream;
     TsdfFrame* dframes = nullptr;
@@ -197,7 +205,7 @@ int surfel_tsdf_eval(long long n_points, const float* points, int n_frames, cons
         // and a stream-ordered free after the kernel.
         const size_t bytes = sizeof(TsdfFrame) * (size_t)n_frames;
         TsdfFrame* host = (TsdfFrame*)malloc(bytes);
-        if (!host) { surfel_set_error("surfel_tsdf_eval: out of host memory"); return 1; }
+        if (!host) { surfel_set_error("%s: out of host memory", who); return 1; }
         for (int f = 0; f < n_frames; f++) {
             const surfel_tsdf_frame_t& F = frames[f];
             const int col[3] = {0, 1, 3};
@@ -212,7 +220,7 @@ int surfel_tsdf_eval(long long n_points, const float* points, int n_frames, cons
         free(host);
         if (e != cudaSuccess) {
             if (dframes) cudaFreeAsync(dframes, st);
-            surfel_set_error("surfel_tsdf_eval: frame table upload failed: %s", cudaGetErrorString(e));
+            surfel_set_error("%s: frame table upload failed: %s", who, cudaGetErrorString(e));
             return 1;
         }
     }
@@ -220,21 +228,47 @@ int surfel_tsdf_eval(long long n_points, const float* points, int n_frames, cons
     {
         LaunchScope scope(kStTsdf, st);
         if (rgb)
-            tsdf_kernel<true><<<(unsigned)blocks, kTsdfThreads, 0, st>>>(n_points, points, n_frames, dframes, depth,
-                                                                         rgb, cx, cy, cz, (float)radius, (float)trunc,
-                                                                         out);
+            tsdf_kernel<true, Points><<<(unsigned)blocks, kTsdfThreads, 0, st>>>(
+                n_points, pts, n_frames, dframes, depth, rgb, cx, cy, cz, (float)radius, (float)trunc, out);
         else
-            tsdf_kernel<false><<<(unsigned)blocks, kTsdfThreads, 0, st>>>(n_points, points, n_frames, dframes, depth,
-                                                                          nullptr, cx, cy, cz, (float)radius,
-                                                                          (float)trunc, out);
+            tsdf_kernel<false, Points><<<(unsigned)blocks, kTsdfThreads, 0, st>>>(
+                n_points, pts, n_frames, dframes, depth, nullptr, cx, cy, cz, (float)radius, (float)trunc, out);
     }
     const cudaError_t launch = cudaGetLastError();
     if (dframes) SURFEL_CUDA_OK(cudaFreeAsync(dframes, st));
     if (launch != cudaSuccess) {
-        surfel_set_error("surfel_tsdf_eval: launch failed: %s", cudaGetErrorString(launch));
+        surfel_set_error("%s: launch failed: %s", who, cudaGetErrorString(launch));
         return 1;
     }
     return 0;
+}
+
+}  // namespace surfel
+
+using namespace surfel;
+
+extern "C" {
+
+int surfel_tsdf_eval(long long n_points, const float* points, int n_frames, const surfel_tsdf_frame_t* frames,
+                     long long map_pixels, const float* depth, const float* rgb, const float* center, double radius,
+                     double trunc, float* out, void* stream) {
+    return tsdf_run("surfel_tsdf_eval", n_points, PointBuffer{points}, points != nullptr, n_frames, frames,
+                    map_pixels, depth, rgb, center, radius, trunc, out, stream);
+}
+
+int surfel_tsdf_eval_grid(int side, const double* bounds, int n_frames, const surfel_tsdf_frame_t* frames,
+                          long long map_pixels, const float* depth, const float* center, double radius, double trunc,
+                          float* out, void* stream) {
+    if (side < 2 || side > kMcMaxSide) {
+        surfel_set_error("surfel_tsdf_eval_grid: side %d outside [2, %d]", side, kMcMaxSide);
+        return 1;
+    }
+    if (!bounds) { surfel_set_error("surfel_tsdf_eval_grid: NULL bounds"); return 1; }
+    PointGrid g;
+    for (int d = 0; d < 3; d++) g.ax[d] = make_lin_axis(bounds[2 * d], bounds[2 * d + 1], side);
+    g.side = side;
+    return tsdf_run("surfel_tsdf_eval_grid", (long long)side * side * side, g, true, n_frames, frames, map_pixels,
+                    depth, nullptr, center, radius, trunc, out, stream);
 }
 
 }  // extern "C"

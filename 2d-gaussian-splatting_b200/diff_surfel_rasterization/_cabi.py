@@ -97,6 +97,19 @@ SIGNATURES = {
     "surfel_tsdf_eval": (c_int, [ctypes.c_longlong, c_void_p, c_int, ctypes.POINTER(TsdfFrame), ctypes.c_longlong,
                                  c_void_p, c_void_p, ctypes.POINTER(c_float), ctypes.c_double, ctypes.c_double,
                                  c_void_p, c_void_p]),
+    "surfel_tsdf_eval_grid": (c_int, [c_int, ctypes.POINTER(ctypes.c_double), c_int, ctypes.POINTER(TsdfFrame),
+                                      ctypes.c_longlong, c_void_p, ctypes.POINTER(c_float), ctypes.c_double,
+                                      ctypes.c_double, c_void_p, c_void_p]),
+    "surfel_mcubes_crop_workspace_bytes": (c_size_t, [c_int]),
+    "surfel_mcubes_crop_count": (c_int, [c_int, c_void_p, ctypes.POINTER(c_int), c_int, c_void_p, c_size_t, c_void_p,
+                                         c_void_p]),
+    "surfel_mcubes_crop_emit": (c_int, [c_int, c_void_p, ctypes.POINTER(ctypes.c_double), ctypes.POINTER(c_int),
+                                        c_int, c_void_p, c_size_t, ctypes.c_longlong, ctypes.c_longlong, c_void_p,
+                                        c_void_p, c_void_p, c_void_p]),
+    "surfel_mcubes_merge_workspace_bytes": (c_size_t, [ctypes.c_longlong]),
+    "surfel_mcubes_merge": (c_int, [ctypes.c_longlong, c_void_p, c_void_p, ctypes.c_longlong, c_void_p, c_int,
+                                    ctypes.POINTER(c_float), ctypes.c_double, c_void_p, c_size_t, c_void_p, c_void_p,
+                                    c_void_p, c_void_p]),
     "surfel_launch_count": (ctypes.c_ulonglong, []),
     "surfel_profile_enable": (None, [c_int]),
     "surfel_profile_num_stages": (c_int, []),

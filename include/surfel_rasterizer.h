@@ -337,6 +337,43 @@ typedef struct surfel_tsdf_frame {
 int surfel_tsdf_eval(long long n_points, const float* points, int n_frames, const surfel_tsdf_frame_t* frames,
                      long long map_pixels, const float* depth, const float* rgb, const float* center, double radius,
                      double trunc, float* out, void* stream);
+/* Grid mode of the field (DESIGN.md §7j): the side^3 points of one crop, torch.linspace(bounds[2d], bounds[2d+1], side)
+ * on each axis d (bounds: 6 host doubles x0, x1, y0, y1, z0, z1, each rounded once to float32) laid out as
+ * meshgrid(indexing="ij") lays them out, x slowest.  out (side^3 floats) is what surfel_tsdf_eval in field mode
+ * returns for those points, without a points buffer.  side in [2, 512]. */
+int surfel_tsdf_eval_grid(int side, const double* bounds, int n_frames, const surfel_tsdf_frame_t* frames,
+                          long long map_pixels, const float* depth, const float* center, double radius, double trunc,
+                          float* out, void* stream);
+
+/* ---- Mesh extraction: marching cubes over contracted crops (marching_cubes_with_contraction of the reference's
+ * utils/mcube_utils.py; rules in DESIGN.md §7j, csrc/mcubes.cu).  The grid is crops_per_axis^3 crops of side^3
+ * points, crop (i, j, k) covering global points [i, j, k] * (side - 1) + [0, side); neighbouring crops share
+ * their boundary plane, which must hold the same values in both.  A corner is inside iff its value is < 0.
+ *  surfel_mcubes_crop_count: counts the crop's vertex records (the crossing edges it owns) and triangles into
+ *   totals[0] and totals[1] (device int64), and keeps per-block offsets in the workspace
+ *   (surfel_mcubes_crop_workspace_bytes(side) bytes, uninitialised is fine).
+ *  surfel_mcubes_crop_emit: with the same arguments and workspace, and the crop's bounds (as in
+ *   surfel_tsdf_eval_grid) and totals, writes n_records vertex keys (uint64) and contracted positions (3 floats
+ *   each), and n_tris triangles as key triples (uint64), in cube order (x slowest) then table order.
+ *  surfel_mcubes_merge: over the records and triangles of all crops, in crop order: writes the distinct keys'
+ *   vertices in ascending key order, uncontracted (DESIGN.md §7i rule 3), scaled by radius, moved by the 3 host
+ *   floats of center and clipped to [-32, 32], to verts (at least n_records rows of 3 floats), their number to
+ *   n_verts (device int64), and each triangle's vertex indices to faces (n_tris rows of 3 int64).  key_bits: the
+ *   bits of the largest key, 4 * G^3 - 1 with G = (side - 1) * crops_per_axis + 1.  n_records must be below 2^30;
+ *   the workspace is surfel_mcubes_merge_workspace_bytes(n_records) bytes (0 when out of range).
+ * All three run on `stream` and do not synchronise; the caller reads the totals to size the outputs. */
+size_t surfel_mcubes_crop_workspace_bytes(int side);
+int surfel_mcubes_crop_count(int side, const float* volume, const int* crop, int crops_per_axis, void* workspace,
+                             size_t workspace_bytes, long long* totals, void* stream);
+int surfel_mcubes_crop_emit(int side, const float* volume, const double* bounds, const int* crop, int crops_per_axis,
+                            const void* workspace, size_t workspace_bytes, long long n_records, long long n_tris,
+                            unsigned long long* vert_keys, float* vert_pos, unsigned long long* tri_keys,
+                            void* stream);
+size_t surfel_mcubes_merge_workspace_bytes(long long n_records);
+int surfel_mcubes_merge(long long n_records, const unsigned long long* vert_keys, const float* vert_pos,
+                        long long n_tris, const unsigned long long* tri_keys, int key_bits, const float* center,
+                        double radius, void* workspace, size_t workspace_bytes, float* verts, long long* faces,
+                        long long* n_verts, void* stream);
 
 /* Instrumentation used by bench.py: number of kernels this library has launched in this process,
  * and optional per-stage CUDA-event timing (events recorded on the launching stream around each
