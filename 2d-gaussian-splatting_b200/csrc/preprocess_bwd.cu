@@ -9,7 +9,8 @@
 //      (dL_dT before step 1 on the scales+rotations path, after it on the transMat_precomp path, as upstream).
 // The kernel writes EVERY output row (zeros for culled splats), so the caller can hand in
 // uninitialised tensors: no separate zero-fill pass over the 59 floats/splat of gradients.
-// Kept quirk (SURVEY A.5): dL_dscale ignores scale_modifier (only the viewer uses modifier != 1).
+// Kept quirk (SURVEY A.5): like upstream, the backward takes L = R diag(s) with scale_modifier fixed to 1, so
+// dL_dscale and the scale-weighted columns 0 and 1 of dL_dR ignore the modifier (only the viewer uses modifier != 1).
 #include "common.cuh"
 #include "kernels.h"
 #include "profile.h"
