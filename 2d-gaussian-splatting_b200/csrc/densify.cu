@@ -5,9 +5,9 @@
 //  * surfel_densify_plan: one pass over the P rows.  Each row's fate depends on that row alone (rules 2, 3
 //    and 7 of §7h never look at the random draw), so the pass decides, per row, whether the original
 //    survives, whether it is cloned and the clone survives, whether it is split and its two copies survive,
-//    and scans four counters across the grid with a single-pass decoupled look-back (as preprocess_fwd.cu's
-//    tile scan): kept originals, kept clones, split rows (all of them: they index the random draw) and kept
-//    split rows.  It stores one int4 per row (the row's rank in each segment, -1 where it has none) and the
+//    and scans four counters across the grid with a single-pass decoupled look-back (scan.cuh): kept
+//    originals, kept clones, split rows (all of them: they index the random draw) and kept split
+//    rows.  It stores one int4 per row (the row's rank in each segment, -1 where it has none) and the
 //    four totals; the caller reads the totals with one device-to-host copy.
 //  * surfel_densify_apply: one launch writes every output row of every group in its table exactly once, params
 //    and both moments, from a by-value table of the groups (like surfel_adam_step); a caller may give the groups
@@ -28,6 +28,7 @@
 #include "../../include/surfel_rasterizer.h"
 #include "common.cuh"
 #include "profile.h"
+#include "scan.cuh"
 
 namespace surfel {
 
@@ -38,7 +39,6 @@ constexpr int kApplyThreads = 256;
 constexpr int kApplyPerThread = 4;
 constexpr int kApplyTile = kApplyThreads * kApplyPerThread;   // floats of one group per apply block
 constexpr int kDensifyMaxP = (1 << 30) - 1;       // P' <= 2P must fit an int32 row index
-constexpr unsigned long long kFlagAgg = 1ull << 32, kFlagPrefix = 2ull << 32;
 
 struct DensifyLayout {
     size_t ctrl, status, rec, total;
@@ -54,15 +54,6 @@ static DensifyLayout densify_layout(int P) {
     L.rec = o;    o = align_up(o + (size_t)(P > 0 ? P : 1) * 16, 256);
     L.total = o;
     return L;
-}
-
-__device__ __forceinline__ unsigned long long ld_status(const unsigned long long* p) {
-    unsigned long long v;
-    asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ void st_status(unsigned long long* p, unsigned long long v) {
-    asm volatile("st.relaxed.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
 }
 
 // torch.max over a dim propagates NaN; fmaxf would drop it
@@ -82,7 +73,7 @@ struct PlanParams {
 __global__ void __launch_bounds__(kPlanThreads) densify_plan_kernel(const __grid_constant__ PlanParams p) {
     __shared__ unsigned long long s_warp[kPlanThreads / 32];
     __shared__ uint32_t s_bid, s_excl[4];
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int tid = threadIdx.x;
     if (tid == 0) s_bid = atomicAdd(&p.ctrl[0], 1u);   // ticket: blocks look back only at blocks already running
     __syncthreads();
     const uint32_t bid = s_bid;
@@ -109,69 +100,20 @@ __global__ void __launch_bounds__(kPlanThreads) densify_plan_kernel(const __grid
             keep_clone = clone && keep_orig;
         }
     }
-    // four 0/1 counters packed in 16-bit fields (block-local sums <= 256): block-wide inclusive scan
+    // four 0/1 counters packed in 16-bit fields (block-local sums <= 256)
     const unsigned long long mine = (unsigned long long)keep_orig | (unsigned long long)keep_clone << 16 |
                                     (unsigned long long)split << 32 | (unsigned long long)keep_split << 48;
-    unsigned long long v = mine;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const unsigned long long n = __shfl_up_sync(0xffffffffu, v, o);
-        if (lane >= o) v += n;
-    }
-    if (lane == 31) s_warp[warp] = v;
-    __syncthreads();
-    if (warp == 0) {
-        unsigned long long w = lane < kPlanThreads / 32 ? s_warp[lane] : 0ull;
-#pragma unroll
-        for (int o = 1; o < kPlanThreads / 32; o <<= 1) {
-            const unsigned long long n = __shfl_up_sync(0xffffffffu, w, o);
-            if (lane >= o) w += n;
-        }
-        if (lane < kPlanThreads / 32) s_warp[lane] = w;
-    }
-    __syncthreads();
-    const unsigned long long block_total = s_warp[kPlanThreads / 32 - 1];
-    const unsigned long long excl_local = v - mine + (warp > 0 ? s_warp[warp - 1] : 0ull);
+    unsigned long long block_total;
+    const unsigned long long excl_local = block_exclusive_scan<kPlanThreads>(mine, s_warp, block_total);
     auto field = [](unsigned long long x, int c) { return (uint32_t)(x >> (16 * c)) & 0xffffu; };
-    const int nb = gridDim.x;
-    if (tid < 4)   // publish this block's aggregate early (its prefix if it is the first block)
-        st_status(p.status + (size_t)tid * nb + bid, (bid == 0 ? kFlagPrefix : kFlagAgg) | field(block_total, tid));
-
-    // ---- decoupled look-back across blocks: warp c scans counter c ----
-    if (warp < 4) {
-        const int c = warp;
-        unsigned long long* status = p.status + (size_t)c * nb;
-        const uint32_t total_c = field(block_total, c);
-        uint32_t excl = 0;
-        if (bid != 0) {
-            int look = (int)bid - 1;
-            while (true) {
-                const int j = look - lane;
-                unsigned long long s = kFlagPrefix;
-                if (j >= 0) {
-                    s = ld_status(status + j);
-                    while ((s >> 32) == 0) s = ld_status(status + j);
-                }
-                const unsigned pm = __ballot_sync(0xffffffffu, (s >> 32) == 2ull);
-                const int first = pm ? (__ffs(pm) - 1) : 32;
-                uint32_t x = (lane <= first) ? (uint32_t)(s & 0xffffffffull) : 0u;
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
-                excl += x;
-                if (pm) break;
-                look -= 32;
-            }
-            if (lane == 0) st_status(status + bid, kFlagPrefix | (unsigned long long)(excl + total_c));
-        }
-        if (lane == 0) {
-            s_excl[c] = excl;
-            if (bid == (uint32_t)nb - 1) p.ctrl[4 + c] = excl + total_c;
-        }
-    }
-    __syncthreads();
-    if (bid == (uint32_t)nb - 1 && tid == 0) {
-        const int ko = (int)p.ctrl[4], kc = (int)p.ctrl[5], s = (int)p.ctrl[6], ks = (int)p.ctrl[7];
-        p.totals[0] = ko; p.totals[1] = kc; p.totals[2] = s; p.totals[3] = ko + kc + 2 * ks;
+    const uint32_t total[4] = {field(block_total, 0), field(block_total, 1), field(block_total, 2),
+                               field(block_total, 3)};
+    block_lookback<4>(p.status, gridDim.x, bid, total, s_excl);
+    if (bid == gridDim.x - 1 && tid == 0) {
+        const uint32_t ko = s_excl[0] + total[0], kc = s_excl[1] + total[1], s = s_excl[2] + total[2],
+                       ks = s_excl[3] + total[3];
+        p.ctrl[4] = ko; p.ctrl[5] = kc; p.ctrl[6] = s; p.ctrl[7] = ks;
+        p.totals[0] = (int)ko; p.totals[1] = (int)kc; p.totals[2] = (int)s; p.totals[3] = (int)(ko + kc + 2 * ks);
     }
     if (i < p.P) {
         int4 r;

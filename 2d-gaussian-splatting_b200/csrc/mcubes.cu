@@ -5,7 +5,7 @@
 //  * surfel_mcubes_crop_count: one thread per grid point of the side^3 crop.  A point counts the crossing edges it
 //    owns (its three edges towards +x, +y, +z; a point on the crop's upper plane belongs to the next crop, unless
 //    this crop is the last along that axis) and, when it is a cube's lower corner, the cube's triangles from the
-//    table.  Both counts are scanned across the grid with a single-pass decoupled look-back (as densify.cu's plan);
+//    table.  Both counts are scanned across the grid with a single-pass decoupled look-back (scan.cuh);
 //    each block keeps its exclusive prefix and the last block writes the crop's two totals, which the caller reads
 //    to size the crop's outputs.
 //  * surfel_mcubes_crop_emit: the same walk, with the block's prefix from the count pass: each crossing edge writes
@@ -28,6 +28,7 @@
 #include "contraction.cuh"
 #include "kernels.h"
 #include "profile.h"
+#include "scan.cuh"
 
 namespace surfel {
 
@@ -38,80 +39,9 @@ namespace {
 constexpr int kMcThreads = 256;
 constexpr int kMcMaxCrops = 1024;                 // crops per axis: keys of (511 * 1024 + 1)^3 * 4 fit 64 bits
 constexpr float kMcMaxRange = 32.f;               // the reference's max_range
-constexpr unsigned long long kFlagAgg = 1ull << 32, kFlagPrefix = 2ull << 32;
 
 // corner k of a cube is at (k & 1, k >> 1 & 1, k >> 2 & 1); edge e runs from kEdgeLo[e] along axis e / 4
 __device__ const unsigned char kEdgeLo[12] = {0, 2, 4, 6, 0, 1, 4, 5, 0, 1, 2, 3};
-
-__device__ __forceinline__ unsigned long long ld_status(const unsigned long long* p) {
-    unsigned long long v;
-    asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ void st_status(unsigned long long* p, unsigned long long v) {
-    asm volatile("st.relaxed.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
-}
-
-// Decoupled look-back of C counters (as densify.cu): block `bid` of `nb` publishes its totals and warp c sums the
-// totals of the blocks before it for counter c into s_excl[c].  Every thread of the block calls it.
-template <int C>
-__device__ __forceinline__ void lookback(unsigned long long* status, int nb, uint32_t bid, const uint32_t* total,
-                                         uint32_t* s_excl) {
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if (tid < C) st_status(status + (size_t)tid * nb + bid, (bid == 0 ? kFlagPrefix : kFlagAgg) | total[tid]);
-    if (warp < C) {
-        unsigned long long* st = status + (size_t)warp * nb;
-        uint32_t excl = 0;
-        if (bid != 0) {
-            int look = (int)bid - 1;
-            while (true) {
-                const int j = look - lane;
-                unsigned long long s = kFlagPrefix;
-                if (j >= 0) {
-                    s = ld_status(st + j);
-                    while ((s >> 32) == 0) s = ld_status(st + j);
-                }
-                const unsigned pm = __ballot_sync(0xffffffffu, (s >> 32) == 2ull);
-                const int first = pm ? (__ffs(pm) - 1) : 32;
-                uint32_t x = (lane <= first) ? (uint32_t)(s & 0xffffffffull) : 0u;
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
-                excl += x;
-                if (pm) break;
-                look -= 32;
-            }
-            if (lane == 0) st_status(st + bid, kFlagPrefix | (unsigned long long)(excl + total[warp]));
-        }
-        if (lane == 0) s_excl[warp] = excl;
-    }
-    __syncthreads();
-}
-
-// Block-wide exclusive scan of a packed value (fields that cannot overflow within a block); returns the thread's
-// exclusive prefix and sets `total` to the block's sum.
-__device__ __forceinline__ uint32_t block_scan(uint32_t mine, uint32_t* s_warp, uint32_t& total) {
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    uint32_t v = mine;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t n = __shfl_up_sync(0xffffffffu, v, o);
-        if (lane >= o) v += n;
-    }
-    if (lane == 31) s_warp[warp] = v;
-    __syncthreads();
-    if (warp == 0) {
-        uint32_t w = lane < kMcThreads / 32 ? s_warp[lane] : 0u;
-#pragma unroll
-        for (int o = 1; o < kMcThreads / 32; o <<= 1) {
-            const uint32_t n = __shfl_up_sync(0xffffffffu, w, o);
-            if (lane >= o) w += n;
-        }
-        if (lane < kMcThreads / 32) s_warp[lane] = w;
-    }
-    __syncthreads();
-    total = s_warp[kMcThreads / 32 - 1];
-    return v - mine + (warp > 0 ? s_warp[warp - 1] : 0u);
-}
 
 struct McCrop {
     const float* vol;      // side^3 values, x slowest
@@ -194,9 +124,9 @@ __global__ void __launch_bounds__(kMcThreads) mc_count_kernel(const __grid_const
     uint32_t mine = 0;
     if (i < n) mine = mc_packed(mc_point(c, i));
     uint32_t packed_total;
-    block_scan(mine, s_warp, packed_total);
+    block_exclusive_scan<kMcThreads>(mine, s_warp, packed_total);
     const uint32_t total[2] = {packed_total & 0xffffu, packed_total >> 16};
-    lookback<2>(w.status, gridDim.x, bid, total, s_excl);
+    block_lookback<2>(w.status, gridDim.x, bid, total, s_excl);
     if (threadIdx.x == 0) {
         w.prefix[bid] = make_uint2(s_excl[0], s_excl[1]);
         if (bid == gridDim.x - 1) {
@@ -220,7 +150,7 @@ __global__ void __launch_bounds__(kMcThreads) mc_emit_kernel(const __grid_consta
         mine = mc_packed(p);
     }
     uint32_t total;
-    const uint32_t excl = block_scan(mine, s_warp, total);
+    const uint32_t excl = block_exclusive_scan<kMcThreads>(mine, s_warp, total);
     if (i >= n || mine == 0) return;
     const uint2 pre = prefix[blockIdx.x];
     const unsigned long long P = gpoint(c, p.l[0], p.l[1], p.l[2]);
@@ -279,8 +209,8 @@ __global__ void __launch_bounds__(kMcThreads) mc_unique_kernel(long long n, cons
     const long long i = (long long)bid * kMcThreads + threadIdx.x;
     const bool first = i < n && (i == 0 || keys[i] != keys[i - 1]);
     uint32_t total;
-    const uint32_t excl = block_scan(first ? 1u : 0u, s_warp, total);
-    lookback<1>(w.status, gridDim.x, bid, &total, s_excl);
+    const uint32_t excl = block_exclusive_scan<kMcThreads>(first ? 1u : 0u, s_warp, total);
+    block_lookback<1>(w.status, gridDim.x, bid, &total, s_excl);
     if (bid == gridDim.x - 1 && threadIdx.x == 0) {
         w.ctrl[1] = s_excl[0] + total;
         *n_verts = (long long)s_excl[0] + total;

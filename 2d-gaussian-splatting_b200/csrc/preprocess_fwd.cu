@@ -5,7 +5,7 @@
 //   near cull -> splat->pixel homography T (in-tree restatement:
 //   /root/reference/gaussian_renderer/__init__.py:64-75) -> view-space normal + dual-visible flip
 //   -> AABB centre/extent -> radius -> tile rect -> SH->RGB (/root/reference/utils/sh_utils.py:57-112)
-// then a block scan of tiles_touched chained across blocks with a decoupled look-back, so the
+// then a block scan of tiles_touched chained across blocks with a decoupled look-back (scan.cuh), so the
 // inclusive offsets and the instance count R come out of the same launch (no separate scan
 // kernel, no second pass over tiles_touched).
 //
@@ -20,6 +20,7 @@
 #include "common.cuh"
 #include "kernels.h"
 #include "profile.h"
+#include "scan.cuh"
 
 namespace surfel {
 
@@ -30,17 +31,6 @@ __constant__ float c_SH_C3[7] = {-0.5900435899266435f, 2.890611442640554f, -0.45
                                  -0.5900435899266435f};
 constexpr float SH_C0 = 0.28209479177387814f;
 constexpr float SH_C1 = 0.4886025119029199f;
-
-constexpr unsigned long long kFlagAgg = 1ull << 32, kFlagPrefix = 2ull << 32;
-
-__device__ __forceinline__ unsigned long long ld_status(const unsigned long long* p) {
-    unsigned long long v;
-    asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ void st_status(unsigned long long* p, unsigned long long v) {
-    asm volatile("st.relaxed.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
-}
 
 __device__ __forceinline__ float sh_eval_channel(const float* sh, int c, int D, float x, float y, float z) {
 #define S(i) sh[3 * (i) + c]
@@ -258,7 +248,7 @@ __global__ void __launch_bounds__(kPreBlock, SURFEL_PRE_BLOCKS) preprocess_fwd_k
         if (w < warp) warp_excl += s;
         block_total += s;
     }
-    if (tid == 0) st_status(p.scan_status + bid, (bid == 0 ? kFlagPrefix : kFlagAgg) | block_total);
+    if (tid == 0) publish_aggregate(p.scan_status, bid, block_total);
 
     // ---- SH -> RGB for surviving splats (rows staged warp-cooperatively) ----
     float rgb[3] = {0, 0, 0};
@@ -429,28 +419,7 @@ __global__ void __launch_bounds__(kPreBlock, SURFEL_PRE_BLOCKS) preprocess_fwd_k
 
     // ---- decoupled look-back across blocks (predecessor aggregates were published early) ----
     if (warp == 0) {
-        unsigned long long* status = p.scan_status;
-        uint32_t excl = 0;
-        if (bid != 0) {
-            int look = (int)bid - 1;
-            while (true) {
-                const int j = look - lane;
-                unsigned long long s = kFlagPrefix;
-                if (j >= 0) {
-                    s = ld_status(status + j);
-                    while ((s >> 32) == 0) s = ld_status(status + j);
-                }
-                const unsigned pm = __ballot_sync(0xffffffffu, (s >> 32) == 2ull);
-                const int first = pm ? (__ffs(pm) - 1) : 32;
-                uint32_t v = (lane <= first) ? (uint32_t)(s & 0xffffffffull) : 0u;
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-                excl += v;
-                if (pm) break;
-                look -= 32;
-            }
-            if (lane == 0) st_status(status + bid, kFlagPrefix | (unsigned long long)(excl + block_total));
-        }
+        const uint32_t excl = warp_lookback(p.scan_status, bid, block_total);
         if (lane == 0) {
             s_excl = excl;
             if (bid == gridDim.x - 1) {
