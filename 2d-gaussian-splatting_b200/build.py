@@ -34,6 +34,7 @@ SOURCES = {
     "densify.cu": ["-fmad=false"],
     "tsdf.cu": ["-fmad=false"],
     "mcubes.cu": ["-fmad=false"],
+    "meshpost.cu": [],
 }
 # Test variants of the library: one render kernel rebuilt with another batch size (slots staged per round), the rest
 # shared with the main library.  tests/test_hitloop_gpu.py runs the whole hit-loop suite against each, so a change

@@ -62,7 +62,8 @@ const char* surfel_profile_stage_name(int stage) {
                                             "sort_onesweep_pass", "identify_tile_ranges", "render_fwd",
                                             "render_bwd", "preprocess_bwd", "mark_visible", "tile_count", "tile_scan",
                                             "tile_scatter", "tile_sort", "adam_step", "densify_stats", "ply_unpack", "ply_pack", "knn", "densify", "tsdf",
-                                            "mcubes_crop", "mcubes_merge"};
+                                            "mcubes_crop", "mcubes_merge", "meshpost_edges", "meshpost_union",
+                                            "meshpost_label", "meshpost_compact"};
     return stage >= 0 && stage < kNumStages ? names[stage] : "";
 }
 int surfel_profile_read(double* ms_out, int* count_out) {

@@ -110,7 +110,13 @@ SIGNATURES = {
     "surfel_mcubes_merge": (c_int, [ctypes.c_longlong, c_void_p, c_void_p, ctypes.c_longlong, c_void_p, c_int,
                                     ctypes.POINTER(c_float), ctypes.c_double, c_void_p, c_size_t, c_void_p, c_void_p,
                                     c_void_p, c_void_p]),
-    "surfel_launch_count": (ctypes.c_ulonglong, []),
+    "surfel_meshpost_workspace_bytes": (c_size_t, [ctypes.c_longlong, ctypes.c_longlong]),
+    "surfel_meshpost_clusters": (c_int, [ctypes.c_longlong, ctypes.c_longlong, c_void_p, c_void_p, c_size_t, c_void_p,
+                                         c_void_p, c_void_p, c_void_p]),
+    "surfel_meshpost_compact": (c_int, [ctypes.c_longlong, ctypes.c_longlong, c_void_p, c_void_p, c_void_p,
+                                        ctypes.c_longlong, ctypes.c_longlong, c_void_p, c_size_t, c_void_p, c_void_p,
+                                        c_void_p, c_void_p]),
+    "surfel_launch_count":(ctypes.c_ulonglong, []),
     "surfel_profile_enable": (None, [c_int]),
     "surfel_profile_num_stages": (c_int, []),
     "surfel_profile_stage_name": (ctypes.c_char_p, [c_int]),

@@ -375,6 +375,30 @@ int surfel_mcubes_merge(long long n_records, const unsigned long long* vert_keys
                         double radius, void* workspace, size_t workspace_bytes, float* verts, long long* faces,
                         long long* n_verts, void* stream);
 
+/* ---- Mesh cluster filtering (post_process_mesh of the reference's utils/mesh_utils.py; rules in DESIGN.md §7k,
+ * csrc/meshpost.cu).  A mesh of n_verts vertices and n_faces faces (rows of 3 int64 vertex indices) on the device;
+ * n_verts below 2^31 and 3 * n_faces below 2^30.  Both calls use a workspace of
+ * surfel_meshpost_workspace_bytes(n_verts, n_faces) bytes (0 when out of range; uninitialised is fine), run on
+ * `stream` and do not synchronise.
+ *  surfel_meshpost_clusters: the faces' connected components over shared edges (unordered vertex-index pairs),
+ *   numbered by the rank of each component's smallest face: each face's cluster id to face_cluster (n_faces int32),
+ *   each cluster's face count to cluster_count[0, C) (n_faces int32 are written), C to info[0] and 1 to info[1] if
+ *   any face index lies outside [0, n_verts), else 0 (info: 2 device int64).  Only when info[1] is 0 do the ids
+ *   and counts mean anything.
+ *  surfel_meshpost_compact: with those ids and counts, C = n_clusters and index in [0, C): keeps the faces whose
+ *   cluster has at least max(the index-th smallest count, 50) faces; writes the old index of each vertex that a kept
+ *   face references, in order, to vert_map (n_verts int64), the kept faces that are not degenerate (three distinct
+ *   indices), in order and renumbered, to out_faces (n_faces rows of 3 int64), and the number of each to info[0]
+ *   and info[1]. */
+size_t surfel_meshpost_workspace_bytes(long long n_verts, long long n_faces);
+int surfel_meshpost_clusters(long long n_verts, long long n_faces, const long long* faces, void* workspace,
+                             size_t workspace_bytes, int* face_cluster, int* cluster_count, long long* info,
+                             void* stream);
+int surfel_meshpost_compact(long long n_verts, long long n_faces, const long long* faces, const int* face_cluster,
+                            const int* cluster_count, long long n_clusters, long long index, void* workspace,
+                            size_t workspace_bytes, long long* out_faces, long long* vert_map, long long* info,
+                            void* stream);
+
 /* Instrumentation used by bench.py: number of kernels this library has launched in this process,
  * and optional per-stage CUDA-event timing (events recorded on the launching stream around each
  * kernel while enabled; surfel_profile_read() waits for them and returns summed ms / launch counts
