@@ -72,9 +72,9 @@ class CudaPipeline:
         return out
 
     # ---- stage 2 ----
-    def _bin_views(self):
+    def _bin_views(self, cap=None):
         offs = (ctypes.c_size_t * 5)()
-        self.lib.surfel_binning_offsets(self.R, self.W, self.H, offs)
+        self.lib.surfel_binning_offsets(self.R if cap is None else cap, self.W, self.H, offs)
         return list(offs)
 
     def duplicate(self):
@@ -89,17 +89,21 @@ class CudaPipeline:
         return dict(keys_unsorted=b[o[0]:o[0] + 8 * R].view(np.uint64).copy(),
                     vals_unsorted=b[o[1]:o[1] + 4 * R].view(np.uint32).copy())
 
-    def bucket(self):
-        """Production binning path (tile buckets + per-tile sort); same outputs as duplicate()+sort()."""
+    def bucket(self, cap=None, fill=0xFF):
+        """Production binning path (tile buckets + per-tile sort); same outputs as duplicate()+sort().
+        cap: instance slots of the workspace (default R), as a capacity-launched forward sizes it; the sorted
+        arrays returned are its first min(R, cap) slots.  fill: byte the workspace is poisoned with (0 makes every
+        slot nobody wrote read as splat 0, a valid index)."""
         lib = self.lib
-        self.binning = torch.full((lib.surfel_binning_bytes(self.R, self.W, self.H),), 0xFF, dtype=torch.uint8, device="cuda")
-        self._check(lib.surfel_bin_bucket(ctypes.byref(self.cs), self.P, self.R, self.geom.data_ptr(),
+        cap = self.R if cap is None else cap
+        self.binning = torch.full((lib.surfel_binning_bytes(cap, self.W, self.H),), fill, dtype=torch.uint8, device="cuda")
+        self._check(lib.surfel_bin_bucket(ctypes.byref(self.cs), self.P, cap, self.geom.data_ptr(),
                                           self.radii.data_ptr(), self.binning.data_ptr(),
                                           self.img.data_ptr() if self.fused_count else None, 1, self.stream))
         torch.cuda.synchronize()
-        o = self._bin_views()
+        o = self._bin_views(cap)
         b = self.binning.cpu().numpy()
-        R, tiles = self.R, self.gx * self.gy
+        R, tiles = min(self.R, cap), self.gx * self.gy
         return dict(keys_sorted=b[o[2]:o[2] + 8 * R].view(np.uint64).copy(),
                     vals_sorted=b[o[3]:o[3] + 4 * R].view(np.uint32).copy(),
                     ranges=b[o[4]:o[4] + 8 * tiles].view(np.uint32).reshape(tiles, 2).copy())
@@ -114,12 +118,13 @@ class CudaPipeline:
                     vals_sorted=b[o[3]:o[3] + 4 * R].view(np.uint32).copy(),
                     ranges=b[o[4]:o[4] + 8 * tiles].view(np.uint32).reshape(tiles, 2).copy())
 
-    def render(self):
+    def render(self, cap=None):
+        """cap: instance slots the binning workspace was laid out for (default R; as passed to bucket())."""
         lib, W, H = self.lib, self.W, self.H
         band = self.cs.tile_row_begin != 0 or self.cs.tile_row_end != 0      # a band leaves the other rows untouched
         fill = 0.0 if band else float("nan")
         self.color = torch.full((3, H, W), fill, device="cuda"); self.others = torch.full((7, H, W), fill, device="cuda")
-        self._check(lib.surfel_render_forward(ctypes.byref(self.cs), self.R, self.geom.data_ptr(),
+        self._check(lib.surfel_render_forward(ctypes.byref(self.cs), self.R if cap is None else cap, self.geom.data_ptr(),
                                               self.binning.data_ptr(), self.img.data_ptr(),
                                               self.color.data_ptr(), self.others.data_ptr(), self.stream))
         torch.cuda.synchronize()
@@ -131,10 +136,10 @@ class CudaPipeline:
                     accum=i[offs[0]:offs[0] + 12 * n].view(np.float32).reshape(3, H, W).copy(),
                     n_contrib=i[offs[1]:offs[1] + 8 * n].view(np.uint32).reshape(2, H, W).copy())
 
-    def backward(self, dL_dcolor, dL_dothers, lowpass_quirk=True, defer_sh=False):
+    def backward(self, dL_dcolor, dL_dothers, lowpass_quirk=True, defer_sh=False, cap=None):
         """defer_sh: surfel_settings.sh_grad_deferred = 1 (dL_dsh left to surfel_sh_grad_expand, which is then
         run here on the kernel's clamp-masked colour gradients; dL_dshs is poisoned first, so a row the expansion
-        misses cannot pass)."""
+        misses cannot pass).  cap: instance slots the binning workspace was laid out for (default R)."""
         lib, P, M = self.lib, self.P, self.M
         self.cs.sh_grad_deferred = int(bool(defer_sh))
         gc, go = _t(dL_dcolor), _t(dL_dothers)
@@ -143,7 +148,7 @@ class CudaPipeline:
         out = dict(dL_dmeans2D=e(P, 3), dL_dcolors=e(P, 3), dL_dopacity=e(P, 1), dL_dmeans3D=e(P, 3),
                    dL_dtransMat=e(P, 9), dL_dshs=e(P, max(M, 1), 3), dL_dscales=e(P, 2), dL_drotations=e(P, 4))
         self._check(lib.surfel_backward(
-            ctypes.byref(self.cs), P, M, self.R, _p(self.means3D), _p(self.scales), _p(self.rotations),
+            ctypes.byref(self.cs), P, M, self.R if cap is None else cap, _p(self.means3D), _p(self.scales), _p(self.rotations),
             _p(self.transMat_precomp), _p(self.shs), int(self.colors_precomp is not None),
             self.radii.data_ptr(), self.geom.data_ptr(), self.binning.data_ptr(), self.img.data_ptr(),
             gc.data_ptr(), go.data_ptr(), scratch.data_ptr(), out["dL_dmeans2D"].data_ptr(),
