@@ -9,6 +9,10 @@ that wants the fused path replaces lines :118-147 of its render() by
 
     out = surface_outputs(allmap, viewpoint_camera, pipe.depth_ratio)
     rets.update(out)
+
+`surface_regularizers(allmap, camera, depth_ratio, lambda_normal, lambda_dist)` goes from `allmap`
+straight to the two regularisers of the reference's train.py (normal consistency and depth distortion),
+two kernels each way with no intermediate plane (see its docstring).
 """
 import torch
 
@@ -68,18 +72,81 @@ class _SurfaceOutputs(torch.autograd.Function):
         return g_allmap, None, None, None
 
 
-def surface_outputs(allmap, viewpoint_camera, depth_ratio):
-    """allmap (7,H,W) from GaussianRasterizer -> dict with the reference's keys."""
+class _SurfaceRegularizers(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, allmap, rot, rays, depth_ratio, lambda_normal, lambda_dist):
+        lib = _cabi.load()
+        allmap = allmap.contiguous().float()
+        _, H, W = allmap.shape
+        dev = allmap.device
+        partials = torch.empty(lib.surfel_post_reg_partials_bytes(W, H) // 8, dtype=torch.float64, device=dev)
+        normal_loss = torch.empty((), device=dev)
+        dist_loss = torch.empty((), device=dev)
+        with torch.cuda.device(dev):
+            _cabi.check(lib.surfel_post_reg_forward(W, H, float(depth_ratio), lambda_normal, lambda_dist,
+                                                    allmap.data_ptr(), rot.data_ptr(), rays.data_ptr(),
+                                                    partials.data_ptr(), normal_loss.data_ptr(), dist_loss.data_ptr(),
+                                                    torch.cuda.current_stream(dev).cuda_stream))
+        ctx.save_for_backward(allmap, rot, rays)
+        ctx.consts = (float(depth_ratio), lambda_normal, lambda_dist)
+        return normal_loss, dist_loss
+
+    @staticmethod
+    def backward(ctx, g_normal, g_dist):
+        lib = _cabi.load()
+        allmap, rot, rays = ctx.saved_tensors
+        depth_ratio, lambda_normal, lambda_dist = ctx.consts
+        _, H, W = allmap.shape
+        dev = allmap.device
+        n = float(W * H)
+        # the cotangents stay on the device (no sync): dL/d(sum over pixels) of each term
+        gscale = torch.stack([g_normal * (lambda_normal / n), g_dist * (lambda_dist / n)]).float().contiguous()
+        tmp = torch.empty((6, H, W), device=dev) if lambda_normal != 0.0 else None
+        g_allmap = torch.empty((7, H, W), device=dev)
+        with torch.cuda.device(dev):
+            _cabi.check(lib.surfel_post_reg_backward(W, H, depth_ratio, lambda_normal, lambda_dist, allmap.data_ptr(),
+                                                     rot.data_ptr(), rays.data_ptr(), gscale.data_ptr(),
+                                                     None if tmp is None else tmp.data_ptr(), g_allmap.data_ptr(),
+                                                     torch.cuda.current_stream(dev).cuda_stream))
+        return g_allmap, None, None, None, None, None
+
+
+def _check_inputs(fn, allmap, viewpoint_camera):
+    """Raise RuntimeError unless allmap is a (7,H,W) CUDA tensor for the camera's size and both camera matrices
+    are (4,4) tensors on its device; returns (W, H)."""
     W, H = int(viewpoint_camera.image_width), int(viewpoint_camera.image_height)
     if not torch.is_tensor(allmap) or not allmap.is_cuda:
-        raise RuntimeError("surface_outputs: allmap must be a CUDA tensor (no CPU path)")
+        raise RuntimeError(f"{fn}: allmap must be a CUDA tensor (no CPU path)")
     if tuple(allmap.shape) != (7, H, W):
-        raise RuntimeError(f"surface_outputs: allmap must be (7, {H}, {W}) for this camera, got {tuple(allmap.shape)}")
+        raise RuntimeError(f"{fn}: allmap must be (7, {H}, {W}) for this camera, got {tuple(allmap.shape)}")
     for name in ("world_view_transform", "full_proj_transform"):
         m = getattr(viewpoint_camera, name)
         if not torch.is_tensor(m) or m.device != allmap.device or tuple(m.shape) != (4, 4):
-            raise RuntimeError(f"surface_outputs: camera {name} must be a (4, 4) tensor on {allmap.device}")
+            raise RuntimeError(f"{fn}: camera {name} must be a (4, 4) tensor on {allmap.device}")
+    return W, H
+
+
+def surface_outputs(allmap, viewpoint_camera, depth_ratio):
+    """allmap (7,H,W) from GaussianRasterizer -> dict with the reference's keys."""
+    W, H = _check_inputs("surface_outputs", allmap, viewpoint_camera)
     rot, rays = _view_matrices(viewpoint_camera.world_view_transform, viewpoint_camera.full_proj_transform, W, H)
     rend_normal, surf_depth, surf_normal = _SurfaceOutputs.apply(allmap, rot, rays, depth_ratio)
     return {"rend_alpha": allmap[1:2], "rend_normal": rend_normal, "rend_dist": allmap[6:7],
             "surf_depth": surf_depth, "surf_normal": surf_normal}
+
+
+def surface_regularizers(allmap, viewpoint_camera, depth_ratio, lambda_normal, lambda_dist):
+    """allmap (7,H,W) from GaussianRasterizer -> (normal_loss, dist_loss), two 0-d float32 CUDA tensors equal to
+    surface_outputs() followed by the reference's train.py regularisers:
+
+        normal_error = (1 - (rend_normal * surf_normal).sum(dim=0))[None]
+        normal_loss = lambda_normal * normal_error.mean()
+        dist_loss = lambda_dist * rend_dist.mean()
+
+    Gradients flow to allmap only; surf_normal's alpha is detached, as in the reference, and where D/alpha is not
+    finite (a hole) its term contributes 0 to the gradient, where the reference's is NaN.  lambda_normal and
+    lambda_dist are Python numbers: lambda_normal == 0 skips the normal term (its loss and gradient are exactly
+    0), and with both 0 nothing reads allmap.  Inputs are checked as surface_outputs checks them."""
+    W, H = _check_inputs("surface_regularizers", allmap, viewpoint_camera)
+    rot, rays = _view_matrices(viewpoint_camera.world_view_transform, viewpoint_camera.full_proj_transform, W, H)
+    return _SurfaceRegularizers.apply(allmap, rot, rays, float(depth_ratio), float(lambda_normal), float(lambda_dist))

@@ -203,6 +203,25 @@ int surfel_post_backward(int W, int H, float depth_ratio, const float* allmap, c
                          const float* g_surf_depth, const float* g_surf_normal, float* tmp6,
                          float* g_allmap, void* stream);
 
+/* OPT-IN fused 2DGS regularisers (SURVEY §8f row f2), straight from allmap with no intermediate plane:
+ *   normal_loss = lambda_normal * mean(1 - sum_c rend_normal_c * surf_normal_c)
+ *   dist_loss   = lambda_dist * mean(rend_dist)
+ * with rend_normal, surf_normal (alpha detached, zero on the border) as surfel_post_forward computes them and
+ * rot / rays as there.  Forward: partials is device scratch of surfel_post_reg_partials_bytes(W, H) bytes
+ * (0 for a bad size); normal_loss and dist_loss are one device float each.  The sums are reduced in double in
+ * a fixed order, so the values are bit-identical from run to run and on any stream.  Backward: gscale2
+ * (device, 2 floats) = (dL/dnormal_loss * lambda_normal / N, dL/ddist_loss * lambda_dist / N), N = W * H;
+ * tmp6 = (6,H,W) scratch, required only when lambda_normal != 0; g_allmap (7,H,W) fully written.  Where
+ * D / alpha is not finite its term contributes 0 to channels 0 and 1.  lambda_normal == 0 skips the stencil
+ * (normal_loss and channels 0-5 exactly 0); with both lambdas 0 nothing reads allmap. */
+size_t surfel_post_reg_partials_bytes(int W, int H);
+int surfel_post_reg_forward(int W, int H, float depth_ratio, double lambda_normal, double lambda_dist,
+                            const float* allmap, const float* rot, const float* rays, double* partials,
+                            float* normal_loss, float* dist_loss, void* stream);
+int surfel_post_reg_backward(int W, int H, float depth_ratio, double lambda_normal, double lambda_dist,
+                             const float* allmap, const float* rot, const float* rays, const float* gscale2,
+                             float* tmp6, float* g_allmap, void* stream);
+
 /* OPT-IN fused photometric loss (SURVEY §8f row f2): (1-l)*L1 + l*(1-SSIM) of
  * /root/reference/train.py:73-74 with /root/reference/utils/loss_utils.py:6-7, :43-73 (11x11 Gaussian
  * window, sigma 1.5, zero padding, per channel).  forward: sums2[0] = sum |img-gt|, sums2[1] = sum of
