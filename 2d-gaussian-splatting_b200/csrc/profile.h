@@ -8,7 +8,8 @@ namespace surfel {
 enum Stage { kStPreFwd = 0, kStDuplicate, kStSortHist, kStSortPass, kStRanges, kStRenderFwd,
              kStRenderBwd, kStPreBwd, kStMarkVisible, kStTileCount, kStTileScan, kStTileScatter,
              kStTileSort, kStAdam, kStDensifyStats, kStPlyUnpack, kStPlyPack, kStKnn, kStDensify, kStTsdf, kStMcubesCrop,
-             kStMcubesMerge, kStMeshpostEdges, kStMeshpostUnion, kStMeshpostLabel, kStMeshpostCompact, kNumStages };
+             kStMcubesMerge, kStMeshpostEdges, kStMeshpostUnion, kStMeshpostLabel, kStMeshpostCompact,
+             kStChamferSample, kStChamferDownsample, kStChamferSelect, kStChamferNn, kNumStages };
 
 void prof_count_launch();
 bool prof_enabled();

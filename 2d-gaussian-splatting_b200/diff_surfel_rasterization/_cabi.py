@@ -121,6 +121,24 @@ SIGNATURES = {
     "surfel_meshpost_compact": (c_int, [ctypes.c_longlong, ctypes.c_longlong, c_void_p, c_void_p, c_void_p,
                                         ctypes.c_longlong, ctypes.c_longlong, c_void_p, c_size_t, c_void_p, c_void_p,
                                         c_void_p, c_void_p]),
+    "surfel_chamfer_max_points": (ctypes.c_longlong, []),
+    "surfel_chamfer_sample_workspace_bytes": (c_size_t, [ctypes.c_longlong]),
+    "surfel_chamfer_sample_count": (c_int, [ctypes.c_longlong, ctypes.c_longlong, c_void_p, c_void_p,
+                                            ctypes.c_double, c_void_p, c_size_t, c_void_p, c_void_p]),
+    "surfel_chamfer_sample_emit": (c_int, [ctypes.c_longlong, ctypes.c_longlong, c_void_p, c_void_p, ctypes.c_double,
+                                           c_void_p, c_size_t, ctypes.c_longlong, c_void_p, c_void_p]),
+    "surfel_chamfer_workspace_bytes": (c_size_t, [ctypes.c_longlong, ctypes.c_longlong]),
+    "surfel_chamfer_downsample": (c_int, [ctypes.c_longlong, ctypes.c_longlong, c_void_p, ctypes.c_double, c_void_p,
+                                          c_size_t, ctypes.POINTER(c_int), c_void_p]),
+    "surfel_chamfer_select": (c_int, [ctypes.c_longlong, ctypes.c_longlong, c_void_p, c_void_p]
+                              + [ctypes.POINTER(ctypes.c_double)] * 3 + [ctypes.c_double, c_void_p,
+                                                                         ctypes.POINTER(c_int),
+                                                                         ctypes.POINTER(ctypes.c_double), c_void_p,
+                                                                         c_size_t] + [c_void_p] * 8),
+    "surfel_chamfer_distances": (c_int, [ctypes.c_longlong, ctypes.c_longlong, c_void_p, ctypes.c_longlong,
+                                         ctypes.c_longlong, c_void_p, ctypes.c_longlong, c_void_p, c_void_p,
+                                         ctypes.c_longlong, c_void_p, c_void_p, ctypes.c_double, ctypes.c_double,
+                                         c_void_p, c_size_t] + [c_void_p] * 6),
     "surfel_launch_count":(ctypes.c_ulonglong, []),
     "surfel_profile_enable": (None, [c_int]),
     "surfel_profile_num_stages": (c_int, []),

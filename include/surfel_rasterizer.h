@@ -418,6 +418,50 @@ int surfel_meshpost_compact(long long n_verts, long long n_faces, const long lon
                             size_t workspace_bytes, long long* out_faces, long long* vert_map, long long* info,
                             void* stream);
 
+/* ---- DTU Chamfer evaluation (scripts/eval_dtu/eval.py of the reference; rules in DESIGN.md §7m, csrc/chamfer.cu).
+ * Everything is float64 rows of 3 on the device; every call runs on `stream`.  Point sets hold at most
+ * surfel_chamfer_max_points() points (the radix sort's limit).
+ *  surfel_chamfer_sample_count: per triangle of the mesh (faces: n_faces rows of 3 int64), the number of points
+ *   the reference's sampling emits at density `thresh`; info (4 device int64): [0] their sum (a triangle beyond the
+ *   limit counts 2^31), [1] 1 if a face index lies outside [0, n_verts), [2] 1 if a vertex coordinate is not finite,
+ *   [3] the number of triangles of positive area.  The workspace is surfel_chamfer_sample_workspace_bytes(n_faces).
+ *  surfel_chamfer_sample_emit: with the same workspace and n_samples = info[0], writes the samples, in triangle and
+ *   row-major order, to rows n_verts .. n_verts + n_samples - 1 of out (rows 0 .. n_verts - 1 are the caller's).
+ *  The next three share one workspace of surfel_chamfer_workspace_bytes(n_points, n_stl) bytes, in this order:
+ *  surfel_chamfer_downsample: the greedy radius-`thresh` downsampling of the (already shuffled) cloud, kept in the
+ *   workspace; synchronises the stream once per eight rounds and returns the number of rounds in *rounds.
+ *  surfel_chamfer_select: the kept points to data_down, those inside [box_lo, box_hi) to data_in, those of data_in
+ *   whose cell rint((x - bb0) / res) of the X*Y*Z mask obs_mask (uint8, C order) is set to data_in_obs with their
+ *   data_down row in obs_down, and the STL points above `plane` to stl_above with their STL row in above_idx
+ *   (every output sized for all points); the four counts to info (4 device int64).
+ *  surfel_chamfer_distances: with those counts (each set non-empty), the distance of each data_in_obs row to the
+ *   STL and of each stl_above row to data_in (+inf at or beyond max_dist) to dist_d2s / dist_s2d, the colours of
+ *   data_down (n_down rows) and of the STL (n_stl rows), and (sum, count) of the distances below max_dist of each
+ *   pass to sums[0..1] and sums[2..3]. */
+long long surfel_chamfer_max_points(void);
+size_t surfel_chamfer_sample_workspace_bytes(long long n_faces);
+int surfel_chamfer_sample_count(long long n_verts, long long n_faces, const double* verts, const long long* faces,
+                                double thresh, void* workspace, size_t workspace_bytes, long long* info,
+                                void* stream);
+int surfel_chamfer_sample_emit(long long n_verts, long long n_faces, const double* verts, const long long* faces,
+                               double thresh, void* workspace, size_t workspace_bytes, long long n_samples,
+                               double* out, void* stream);
+size_t surfel_chamfer_workspace_bytes(long long n_points, long long n_stl);
+int surfel_chamfer_downsample(long long n_points, long long n_stl, const double* pcd, double thresh,
+                              void* workspace, size_t workspace_bytes, int* rounds, void* stream);
+int surfel_chamfer_select(long long n_points, long long n_stl, const double* pcd, const double* stl,
+                          const double* box_lo, const double* box_hi, const double* bb0, double res,
+                          const unsigned char* obs_mask, const int* obs_shape, const double* plane, void* workspace,
+                          size_t workspace_bytes, double* data_down, double* data_in, double* data_in_obs,
+                          unsigned int* obs_down, double* stl_above, unsigned int* above_idx, long long* info,
+                          void* stream);
+int surfel_chamfer_distances(long long n_points, long long n_stl, const double* stl, long long n_down, long long n_in,
+                             const double* data_in, long long n_obs, const double* data_in_obs,
+                             const unsigned int* obs_down, long long n_above, const double* stl_above,
+                             const unsigned int* above_idx, double max_dist, double vis, void* workspace,
+                             size_t workspace_bytes, double* dist_d2s, double* dist_s2d, double* data_color,
+                             double* stl_color, double* sums, void* stream);
+
 /* Instrumentation used by bench.py: number of kernels this library has launched in this process,
  * and optional per-stage CUDA-event timing (events recorded on the launching stream around each
  * kernel while enabled; surfel_profile_read() waits for them and returns summed ms / launch counts
