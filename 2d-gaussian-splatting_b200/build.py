@@ -36,6 +36,7 @@ SOURCES = {
     "mcubes.cu": ["-fmad=false"],
     "meshpost.cu": [],
     "chamfer.cu": ["-fmad=false"],
+    "cull.cu": ["-fmad=false"],
 }
 # Test variants of the library: one render kernel rebuilt with another batch size (slots staged per round), the rest
 # shared with the main library.  tests/test_hitloop_gpu.py runs the whole hit-loop suite against each, so a change

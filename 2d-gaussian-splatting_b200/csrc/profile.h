@@ -9,7 +9,8 @@ enum Stage { kStPreFwd = 0, kStDuplicate, kStSortHist, kStSortPass, kStRanges, k
              kStRenderBwd, kStPreBwd, kStMarkVisible, kStTileCount, kStTileScan, kStTileScatter,
              kStTileSort, kStAdam, kStDensifyStats, kStPlyUnpack, kStPlyPack, kStKnn, kStDensify, kStTsdf, kStMcubesCrop,
              kStMcubesMerge, kStMeshpostEdges, kStMeshpostUnion, kStMeshpostLabel, kStMeshpostCompact,
-             kStChamferSample, kStChamferDownsample, kStChamferSelect, kStChamferNn, kNumStages };
+             kStChamferSample, kStChamferDownsample, kStChamferSelect, kStChamferNn,
+             kStCullDilate, kStCullVertices, kStCullFaces, kStCullEmit, kNumStages };
 
 void prof_count_launch();
 bool prof_enabled();

@@ -139,6 +139,17 @@ SIGNATURES = {
                                          ctypes.c_longlong, c_void_p, ctypes.c_longlong, c_void_p, c_void_p,
                                          ctypes.c_longlong, c_void_p, c_void_p, ctypes.c_double, ctypes.c_double,
                                          c_void_p, c_size_t] + [c_void_p] * 6),
+    "surfel_cull_max_views": (c_int, []),
+    "surfel_cull_max_radius": (c_int, []),
+    "surfel_cull_workspace_bytes": (c_size_t, [ctypes.c_longlong, c_int, c_int, ctypes.c_longlong,
+                                               ctypes.c_longlong]),
+    "surfel_cull_dilate": (c_int, [c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p, c_void_p]),
+    "surfel_cull_vertices": (c_int, [ctypes.c_longlong, c_void_p, ctypes.c_longlong, c_void_p, c_int, c_void_p,
+                                     c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p, c_void_p,
+                                     c_void_p]),
+    "surfel_cull_emit": (c_int, [ctypes.c_longlong, c_void_p, ctypes.c_longlong, c_void_p,
+                                 ctypes.POINTER(ctypes.c_double), c_void_p, ctypes.c_longlong, c_void_p, c_size_t,
+                                 ctypes.c_longlong, ctypes.c_longlong, c_void_p, c_void_p, c_void_p, c_void_p]),
     "surfel_launch_count":(ctypes.c_ulonglong, []),
     "surfel_profile_enable": (None, [c_int]),
     "surfel_profile_num_stages": (c_int, []),

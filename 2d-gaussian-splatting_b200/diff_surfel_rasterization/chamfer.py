@@ -10,6 +10,11 @@ Every step is float64 and reproduces the reference's evaluation order bit for bi
 radius downsampling, the float32 box, the observation grid, the plane, the colours) are in DESIGN.md §7m.  The only
 randomness is the shuffle: pass `perm` for the reference's order, or it is drawn on the device from `generator`.
 No CPU path.
+
+The step before it, the DTU mask culling of scripts/eval_dtu/evaluate_single_scene.py (cull_scan, lines 19-101), is
+here too (csrc/cull.cu, DESIGN.md §7n):
+
+    v, f, c = cull_scan(verts, faces, masks, world_mats, scale_mats, colors=None)   # then sample_mesh(v, f)
 """
 import ctypes
 import math
@@ -206,3 +211,105 @@ def dtu_chamfer(pcd, stl, obs_mask, bb, res, plane, perm=None, generator=None, d
         mean_s2d = s_s2d / c_s2d if c_s2d else math.nan
         return ChamferResult(mean_d2s, mean_s2d, (mean_d2s + mean_s2d) / 2, down[:n_down], data_color, stl_color,
                              dist_d2s, dist_s2d, rounds.value)
+
+
+def dtu_projections(world_mats, scale_mats):
+    """The projection cull_scan uses for each DTU view (DESIGN.md §7n, rule 1): (N,3,4) float32 host array, rows 0-2
+    of intrinsics @ inverse(pose) as the reference's evaluate_single_scene.py builds them from P = (world_mat @
+    scale_mat)[:3, :4] with cv2.decomposeProjectionMatrix.  That product is sign(det P[:, :3]) * P / |P[2, :3]|, which
+    is evaluated here in float64 and rounded once.  world_mats, scale_mats: the (N,4,4) matrices of cameras.npz, as
+    host arrays or tensors.  ValueError on other shapes, non-finite entries or a singular P[:, :3]."""
+    who = "dtu_projections"
+    wm, sm = _host(world_mats, np.float32), _host(scale_mats, np.float32)
+    if wm.ndim != 3 or wm.shape[1:] != (4, 4) or sm.shape != wm.shape:
+        raise ValueError(f"{who}: world_mats and scale_mats must both be (N,4,4), got {wm.shape} and {sm.shape}")
+    # world_mat @ scale_mat in float32, one view at a time, as the reference forms it
+    P = np.stack([w @ s for w, s in zip(wm, sm)])[:, :3, :4].astype(np.float64) if len(wm) else np.zeros((0, 3, 4))
+    det = np.linalg.det(P[:, :, :3]) if len(P) else np.zeros(0)
+    norm = np.sqrt((P[:, 2, :3] ** 2).sum(1))
+    if not (np.isfinite(P).all() and np.isfinite(det).all() and (det != 0).all() and (norm > 0).all()):
+        raise ValueError(f"{who}: a camera matrix is not finite or P[:, :3] is singular")
+    return (np.sign(det)[:, None, None] * P / norm[:, None, None]).astype(np.float32)
+
+
+def _cull(who, verts, faces, masks, proj, scale_mats, colors, image_size, radius):
+    """cull_scan with the projections given: dict of the outputs, the bit-packed dilated masks and the keep flags."""
+    _cuda(who, "masks", masks)
+    if masks.dtype not in (torch.uint8, torch.bool) or masks.dim() != 3:
+        raise ValueError(f"{who}: masks must be (N,H,W) uint8 or bool, got {tuple(masks.shape)} {masks.dtype}")
+    dev = masks.device
+    v = _points(who, "verts", verts, dev)
+    _cuda(who, "faces", faces)
+    if faces.dtype not in (torch.int32, torch.int64) or faces.dim() != 2 or faces.shape[1] != 3 or faces.device != dev:
+        raise ValueError(f"{who}: faces must be (F,3) int32 or int64 on {dev}, got {tuple(faces.shape)} "
+                         f"{faces.dtype} on {faces.device}")
+    M, F = v.shape[0], faces.shape[0]
+    if colors is not None:
+        _cuda(who, "colors", colors)
+        if colors.dim() != 2 or colors.shape[0] != M or colors.device != dev:
+            raise ValueError(f"{who}: colors must be ({M},C) on {dev}, got {tuple(colors.shape)} on {colors.device}")
+    size = tuple(int(s) for s in image_size)
+    if len(size) != 2 or min(size) < 1:
+        raise ValueError(f"{who}: image_size must be (W, H) with positive sides, got {image_size}")
+    lib = _cabi.load()
+    if isinstance(radius, bool) or int(radius) != radius or not 0 <= radius <= lib.surfel_cull_max_radius():
+        raise ValueError(f"{who}: radius must be an integer in [0, {lib.surfel_cull_max_radius()}], got {radius}")
+    radius = int(radius)
+    N, H, W = masks.shape
+    if proj.shape != (N, 3, 4):
+        raise ValueError(f"{who}: {N} masks and {proj.shape[0]} cameras")
+    if not 1 <= N <= lib.surfel_cull_max_views():
+        raise ValueError(f"{who}: {N} views; 1 to {lib.surfel_cull_max_views()} are supported")
+    sm0 = _host(scale_mats, np.float32).reshape(-1, 4, 4)[0]
+    world = (ctypes.c_double * 4)(float(sm0[0, 0]), float(sm0[0, 3]), float(sm0[1, 3]), float(sm0[2, 3]))
+    ws_bytes = lib.surfel_cull_workspace_bytes(N, H, W, M, F)
+    if ws_bytes == 0:
+        raise ValueError(f"{who}: {N} masks of {W} x {H}, {M} vertices and {F} faces; sides up to 32768 and up to "
+                         f"2^31 - 1 vertices and faces are supported")
+    with torch.cuda.device(dev):
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        m8 = masks.contiguous().view(torch.uint8)
+        f = faces.to(torch.int64).contiguous()
+        A = torch.from_numpy(np.ascontiguousarray(proj, np.float32)).to(dev)
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+        dilated = torch.empty((N, H, (W + 31) // 32), dtype=torch.int32, device=dev)
+        keep = torch.empty(M, dtype=torch.uint8, device=dev)
+        info = torch.empty(4, dtype=torch.int64, device=dev)
+        _cabi.check(lib.surfel_cull_dilate(N, H, W, radius, m8.data_ptr(), ws.data_ptr(), ws_bytes,
+                                           dilated.data_ptr(), stream))
+        _cabi.check(lib.surfel_cull_vertices(M, v.data_ptr(), F, f.data_ptr(), N, A.data_ptr(), size[0], size[1], H,
+                                             W, dilated.data_ptr(), ws.data_ptr(), ws_bytes, keep.data_ptr(),
+                                             info.data_ptr(), stream))
+        bad, nonfinite, n_verts, n_faces = info.tolist()
+        if bad:
+            raise ValueError(f"{who}: a face index lies outside [0, {M})")
+        if nonfinite:
+            raise ValueError(f"{who}: verts contain a coordinate that is not finite in float32")
+        out_v = torch.empty((n_verts, 3), dtype=torch.float64, device=dev)
+        out_f = torch.empty((n_faces, 3), dtype=torch.int64, device=dev)
+        c = None if colors is None else colors.contiguous()
+        out_c = None if c is None else torch.empty((n_verts, c.shape[1]), dtype=c.dtype, device=dev)
+        row_bytes = 0 if c is None else c.shape[1] * c.element_size()
+        _cabi.check(lib.surfel_cull_emit(M, v.data_ptr(), F, f.data_ptr(), world, 0 if c is None else c.data_ptr(),
+                                         row_bytes, ws.data_ptr(), ws_bytes, n_verts, n_faces, out_v.data_ptr(),
+                                         out_f.data_ptr(),
+                                         0 if out_c is None else out_c.data_ptr(), stream))
+        return dict(verts=out_v, faces=out_f, colors=out_c, dilated=dilated, keep=keep.bool())
+
+
+@torch.no_grad()
+def cull_scan(verts, faces, masks, world_mats, scale_mats, colors=None, image_size=(1600, 1200), radius=24):
+    """The reference's DTU mask culling (cull_scan of scripts/eval_dtu/evaluate_single_scene.py, DESIGN.md §7n), the
+    step before eval.py scores a mesh: drops every vertex that some view projects inside the image_size (W, H) frame
+    onto a pixel outside that view's mask dilated by disk(radius), drops every face that lost a vertex and maps the
+    rest to world units with scale_mats[0].
+
+    verts (M,3) float32 or float64, faces (F,3) int32 or int64, colors None or (M,C), masks (N,H,W) uint8 or bool
+    (channel 0 of each mask image; nonzero is set), all on one CUDA device; world_mats and scale_mats: the (N,4,4)
+    matrices of cameras.npz.  Returns (verts (M',3) float64, faces (F',3) int64, colours (M',C) or None): kept
+    vertices in order (unreferenced ones included) and kept faces renumbered.  Runs on the current stream; the inputs
+    are not changed.  ValueError on a face index outside [0, M), a vertex that is not finite in float32, masks and
+    cameras that disagree in N, or sizes beyond the supported counts."""
+    r = _cull("cull_scan", verts, faces, masks, dtu_projections(world_mats, scale_mats), scale_mats, colors,
+              image_size, radius)
+    return r["verts"], r["faces"], r["colors"]

@@ -462,6 +462,36 @@ int surfel_chamfer_distances(long long n_points, long long n_stl, const double* 
                              size_t workspace_bytes, double* dist_d2s, double* dist_s2d, double* data_color,
                              double* stl_color, double* sums, void* stream);
 
+/* ---- DTU mask culling (cull_scan of the reference's scripts/eval_dtu/evaluate_single_scene.py; rules in DESIGN.md
+ * §7n, csrc/cull.cu).  n_views masks of height x width bytes (C order, nonzero = set), 1 <= n_views <=
+ * surfel_cull_max_views(), each side in [1, 32768]; meshes of at most 2^31 - 1 vertices and faces.  One workspace of
+ * surfel_cull_workspace_bytes(n_views, height, width, n_verts, n_faces) bytes (0 when out of range; uninitialised is
+ * fine) serves the three calls, in this order; each runs on `stream` and does not synchronise.
+ *  surfel_cull_dilate: each mask dilated by disk(radius) with a zero border, 0 <= radius <= surfel_cull_max_radius(),
+ *   bit-packed to dilated: n_views * height rows of ceil(width / 32) words, pixel x of a row in bit x % 32 of word
+ *   x / 32, bits beyond the width clear.
+ *  surfel_cull_vertices: verts (n_verts rows of 3 float64) against the dilated masks through proj (n_views rows of
+ *   3 x 4 float32, device) with the image size image_width x image_height: 1 or 0 per vertex to keep (n_verts bytes);
+ *   info (4 device int64): [0] 1 if a face index (faces: n_faces rows of 3 int64) lies outside [0, n_verts), [1] 1 if
+ *   a vertex coordinate is not finite in float32, [2] the kept vertices, [3] the kept faces (all three vertices kept).
+ *  surfel_cull_emit: with the same workspace and n_kept_verts = info[2], n_kept_faces = info[3], the kept vertices
+ *   in order as v * world[0] + world[1..3] (float64, world: 4 host doubles) to out_verts (n_kept_verts rows of 3),
+ *   their colour rows (color_row_bytes each, 0 for none) to out_colors, and the kept faces in order, renumbered, to
+ *   out_faces (n_kept_faces rows of 3 int64).  Outputs with nothing to hold may be NULL. */
+int surfel_cull_max_views(void);
+int surfel_cull_max_radius(void);
+size_t surfel_cull_workspace_bytes(long long n_views, int height, int width, long long n_verts, long long n_faces);
+int surfel_cull_dilate(int n_views, int height, int width, int radius, const unsigned char* masks, void* workspace,
+                       size_t workspace_bytes, unsigned int* dilated, void* stream);
+int surfel_cull_vertices(long long n_verts, const double* verts, long long n_faces, const long long* faces,
+                         int n_views, const float* proj, int image_width, int image_height, int height, int width,
+                         const unsigned int* dilated, void* workspace, size_t workspace_bytes, unsigned char* keep,
+                         long long* info, void* stream);
+int surfel_cull_emit(long long n_verts, const double* verts, long long n_faces, const long long* faces,
+                     const double* world, const void* colors, long long color_row_bytes, const void* workspace,
+                     size_t workspace_bytes, long long n_kept_verts, long long n_kept_faces, double* out_verts,
+                     long long* out_faces, void* out_colors, void* stream);
+
 /* Instrumentation used by bench.py: number of kernels this library has launched in this process,
  * and optional per-stage CUDA-event timing (events recorded on the launching stream around each
  * kernel while enabled; surfel_profile_read() waits for them and returns summed ms / launch counts
