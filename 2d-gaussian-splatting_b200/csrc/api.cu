@@ -51,40 +51,30 @@ bool frame_of(const surfel_settings_t* s, Frame& f) {
     return true;
 }
 
-int tile_key_bits(int tiles) {   // 32 depth bits + (index of highest set bit of tiles) + 1
-    int b = 0;
-    unsigned n = (unsigned)tiles;
-    while (n) { b++; n >>= 1; }
-    return 32 + b;
-}
+// keys are tile << 32 | depth bits; the width covers tile indices up to `tiles` itself
+int tile_key_bits(int tiles) { return radix_key_bits((unsigned long long)(unsigned)tiles << 32 | 0xffffffffull); }
+
+size_t binning_pairs(size_t R) { return R > 0 ? R : 1; }
 
 BinningLayout binning_layout(size_t R, int tiles) {
     BinningLayout L;
-    size_t r = R > 0 ? R : 1, o = 0;
-    L.keys_a = o;    o = align_up(o + r * 8, 256);
-    L.keys_b = o;    o = align_up(o + r * 8, 256);
-    L.vals_a = o;    o = align_up(o + r * 4, 256);
-    L.vals_b = o;    o = align_up(o + r * 4, 256);
-    L.ranges = o;    o = align_up(o + (size_t)tiles * 8, 256);
-    L.sort_temp = o; o = align_up(o + std::max(radix_sort_temp_bytes(r), bucket_temp_bytes(tiles)), 256);
+    const size_t r = binning_pairs(R);
+    size_t o = 0;
+    L.pairs = o;  o = align_up(o + radix_sort_pairs_bytes(r), 256);
+    L.ranges = o; o = align_up(o + (size_t)tiles * 8, 256);
+    L.temp = o;   o = align_up(o + std::max(radix_sort_temp_bytes(r), bucket_temp_bytes(tiles)), 256);
     L.total = o;
     return L;
 }
 
-struct BinView { uint64_t *k_unsorted, *k_sorted; uint32_t *v_unsorted, *v_sorted; uint64_t *k_a, *k_b; uint32_t *v_a, *v_b; uint2* ranges; void* temp; };
+// sort.in: duplicated keys and values; sort.out: the sorted ones, whichever sort bins them
+struct BinView { RadixSortWs sort; uint2* ranges; };
 
-BinView bin_view(void* ws, size_t R, const Frame& f) {
-    BinningLayout L = binning_layout(R, f.tiles);
+BinView bin_view(void* ws, size_t R, int tiles) {
+    const BinningLayout L = binning_layout(R, tiles);
     char* c = (char*)ws;
-    BinView v;
-    v.k_a = (uint64_t*)(c + L.keys_a); v.k_b = (uint64_t*)(c + L.keys_b);
-    v.v_a = (uint32_t*)(c + L.vals_a); v.v_b = (uint32_t*)(c + L.vals_b);
-    const bool in_b = radix_sort_passes(tile_key_bits(f.tiles)) & 1;
-    v.k_unsorted = v.k_a; v.v_unsorted = v.v_a;
-    v.k_sorted = in_b ? v.k_b : v.k_a; v.v_sorted = in_b ? v.v_b : v.v_a;
-    v.ranges = (uint2*)(c + L.ranges);
-    v.temp = c + L.sort_temp;
-    return v;
+    return BinView{radix_sort_ws(c + L.pairs, binning_pairs(R), tile_key_bits(tiles), c + L.temp),
+                   (uint2*)(c + L.ranges)};
 }
 
 // Device-visible alias of a pinned (cudaHostAlloc / cudaHostRegister, mapped) host word, or nullptr
@@ -137,11 +127,10 @@ int surfel_geom_offsets(int P, size_t* out) {
 }
 int surfel_binning_offsets(size_t R, int W, int H, size_t* out) {
     const int tiles = ((W + kBlockX - 1) / kBlockX) * ((H + kBlockY - 1) / kBlockY);
-    BinningLayout L = binning_layout(R, tiles);
-    const bool in_b = radix_sort_passes(tile_key_bits(tiles)) & 1;
-    out[0] = L.keys_a; out[1] = L.vals_a;
-    out[2] = in_b ? L.keys_b : L.keys_a; out[3] = in_b ? L.vals_b : L.vals_a;
-    out[4] = L.ranges;
+    const BinView v = bin_view(nullptr, R, tiles);   // at base 0 every address is an offset
+    out[0] = (size_t)v.sort.in.keys; out[1] = (size_t)v.sort.in.vals;
+    out[2] = (size_t)v.sort.out.keys; out[3] = (size_t)v.sort.out.vals;
+    out[4] = (size_t)v.ranges;
     return 0;
 }
 int surfel_image_offsets(int W, int H, size_t* out) {
@@ -196,19 +185,18 @@ int surfel_bin_duplicate(const surfel_settings_t* s, int P, uint32_t R, const vo
     if (R == 0 || P == 0) return 0;
     GeomLayout L = geom_layout(P);
     const char* g = (const char*)geom_ws;
-    BinView v = bin_view(binning_ws, R, f);
+    BinView v = bin_view(binning_ws, R, f.tiles);
     return launch_duplicate_with_keys(P, f.gx, f.gy, f.row0, f.row1, (const float4*)(g + L.tmat), radii,
-                                      (const uint32_t*)(g + L.offsets), v.k_unsorted, v.v_unsorted,
+                                      (const uint32_t*)(g + L.offsets), v.sort.in.keys, v.sort.in.vals,
                                       (cudaStream_t)stream);
 }
 
 int surfel_bin_sort(const surfel_settings_t* s, uint32_t R, void* binning_ws, void* stream) {
     Frame f;
     if (!frame_of(s, f)) return 1;
-    BinView v = bin_view(binning_ws, R, f);
-    if (launch_radix_sort_pairs(v.k_a, v.v_a, v.k_b, v.v_b, R, tile_key_bits(f.tiles), v.temp,
-                                (cudaStream_t)stream)) return 1;
-    return launch_identify_tile_ranges(R, f.tiles, v.k_sorted, v.ranges, (cudaStream_t)stream);
+    BinView v = bin_view(binning_ws, R, f.tiles);
+    if (launch_radix_sort_pairs(v.sort, R, (cudaStream_t)stream)) return 1;
+    return launch_identify_tile_ranges(R, f.tiles, v.sort.out.keys, v.ranges, (cudaStream_t)stream);
 }
 
 int surfel_render_forward(const surfel_settings_t* s, uint32_t R, const void* geom_ws,
@@ -216,12 +204,12 @@ int surfel_render_forward(const surfel_settings_t* s, uint32_t R, const void* ge
                           float* out_others, void* stream) {
     Frame f;
     if (!frame_of(s, f)) return 1;
-    BinView v = bin_view(const_cast<void*>(binning_ws), R, f);
+    BinView v = bin_view(const_cast<void*>(binning_ws), R, f.tiles);
     ImageLayout I = image_layout(f.W, f.H);
     RenderParams p;
     memset(&p, 0, sizeof(p));
     p.W = f.W; p.H = f.H; p.gx = f.gx; p.gy = f.gy; p.row0 = f.row0; p.row1 = f.row1;
-    p.ranges = v.ranges; p.point_list = v.v_sorted;
+    p.ranges = v.ranges; p.point_list = v.sort.out.vals;
     p.rec = (const float4*)((const char*)geom_ws + 0);   // records sit at offset 0 of the geometry workspace
     p.bg = s->bg;
     p.out_color = out_color; p.out_others = out_others;
@@ -248,12 +236,12 @@ int surfel_bin_bucket(const surfel_settings_t* s, int P, uint32_t R, const void*
     if (!frame_of(s, f)) return 1;
     GeomLayout L = geom_layout(P);
     const char* g = (const char*)geom_ws;
-    BinView v = bin_view(binning_ws, R, f);
-    // scratch pairs live in whichever key buffer does NOT receive the sorted keys
-    unsigned long long* pairs = (unsigned long long*)(v.k_sorted == v.k_a ? v.k_b : v.k_a);
+    BinView v = bin_view(binning_ws, R, f.tiles);
+    // the same result buffers as the radix sort's; its spare keys hold the scratch pairs
     return launch_bucket_binning(P, R, f.gx, f.gy, f.row0, f.row1, (const float4*)(g + L.tmat), radii,
-                                 (const uint32_t*)(g + L.offsets), pairs, v.v_sorted,
-                                 write_keys ? (unsigned long long*)v.k_sorted : nullptr, v.ranges, v.temp,
+                                 (const uint32_t*)(g + L.offsets), (unsigned long long*)v.sort.spare.keys,
+                                 v.sort.out.vals, write_keys ? (unsigned long long*)v.sort.out.keys : nullptr,
+                                 v.ranges, v.sort.temp,
                                  image_ws_with_counts ? (const uint32_t*)((const char*)image_ws_with_counts +
                                                                           image_layout(f.W, f.H).tile_count) : nullptr,
                                  (cudaStream_t)stream);
@@ -290,12 +278,12 @@ int surfel_backward(const surfel_settings_t* s, int P, int M, uint32_t R, const 
     const char* g = (const char*)geom_ws;
     SURFEL_CUDA_OK(cudaMemsetAsync(grad_scratch, 0, (size_t)P * kGradFloats * 4, st));
     if (R > 0) {
-        BinView v = bin_view(const_cast<void*>(binning_ws), R, f);
+        BinView v = bin_view(const_cast<void*>(binning_ws), R, f.tiles);
         ImageLayout I = image_layout(f.W, f.H);
         RenderParams p;
         memset(&p, 0, sizeof(p));
         p.W = f.W; p.H = f.H; p.gx = f.gx; p.gy = f.gy; p.row0 = f.row0; p.row1 = f.row1;
-        p.ranges = v.ranges; p.point_list = v.v_sorted; p.rec = (const float4*)(g + L.rec); p.bg = s->bg;
+        p.ranges = v.ranges; p.point_list = v.sort.out.vals; p.rec = (const float4*)(g + L.rec); p.bg = s->bg;
         p.accum = (float*)((char*)image_ws + I.accum); p.n_contrib = (uint32_t*)((char*)image_ws + I.n_contrib);
         p.dL_dpix = dL_dout_color; p.dL_dothers = dL_dout_others; p.grad_rec = grad_scratch;
         p.grad_plane = s->grad_plane_stride > 0 ? (size_t)s->grad_plane_stride : (size_t)f.W * f.H;
@@ -338,8 +326,9 @@ int surfel_grad_scratch_floats(void) { return kGradFloats; }
 
 int surfel_sort_pairs(uint64_t* keys_a, uint32_t* vals_a, uint64_t* keys_b, uint32_t* vals_b,
                       size_t n, int end_bit, void* temp, int* result_in_b, void* stream) {
-    if (result_in_b) *result_in_b = radix_sort_passes(end_bit) & 1;
-    return launch_radix_sort_pairs(keys_a, vals_a, keys_b, vals_b, n, end_bit, temp, (cudaStream_t)stream);
+    const RadixSortWs ws = radix_sort_ws(SortPairs{keys_a, vals_a}, SortPairs{keys_b, vals_b}, temp, end_bit);
+    if (result_in_b) *result_in_b = ws.out.keys != keys_a;
+    return launch_radix_sort_pairs(ws, n, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -40,7 +40,7 @@ namespace {
 constexpr int kChThreads = 256;
 constexpr int kBox = 32;                          // points per level-0 box == lanes per warp
 constexpr int kMaxLevels = 8;                     // 32^7 boxes of 32 points > 2^30 points
-constexpr long long kChMaxPoints = (1ll << 30) - 1;   // the radix sort's limit; indices fit in u32
+constexpr long long kChMaxPoints = kRadixSortMaxPairs;   // indices fit in u32
 constexpr int kRoundBatch = 8;                    // greedy rounds launched per read of the undecided count
 constexpr uint8_t kUndecided = 0, kKept = 1, kRemoved = 2;
 
@@ -719,8 +719,8 @@ SampleLayout sample_layout(long long F) {
 
 // evaluation workspace for a cloud of N points and an STL of S points; T = max(N, S)
 struct EvalLayout {
-    size_t ctrl, rounds, status_n, status_s, ka, kb, va, vb, temp, state, pts_a, boxes_a, pts_b, boxes_b, pts_q,
-        partial, total;
+    size_t ctrl, rounds, status_n, status_s, sort, state, pts_a, boxes_a, pts_b, boxes_b, pts_q, partial, total;
+    size_t t;   // pairs the sort has room for
 };
 EvalLayout eval_layout(long long N, long long S) {
     EvalLayout L;
@@ -730,11 +730,7 @@ EvalLayout eval_layout(long long N, long long S) {
     L.rounds = o;   o = align_up(o + kRoundBatch * 4, 256);
     L.status_n = o; o = align_up(o + (size_t)3 * blocks_of(N) * 8, 256);
     L.status_s = o; o = align_up(o + (size_t)blocks_of(S) * 8, 256);
-    L.ka = o;       o = align_up(o + t * 8, 256);
-    L.kb = o;       o = align_up(o + t * 8, 256);
-    L.va = o;       o = align_up(o + t * 4, 256);
-    L.vb = o;       o = align_up(o + t * 4, 256);
-    L.temp = o;     o = align_up(o + radix_sort_temp_bytes(t), 256);
+    L.sort = o;     o = align_up(o + radix_sort_workspace_bytes(t), 256);
     L.state = o;    o = align_up(o + n, 256);
     L.pts_a = o;    o = align_up(o + n * 32, 256);
     L.boxes_a = o;  o = align_up(o + boxes_for(n) * 64, 256);
@@ -743,6 +739,7 @@ EvalLayout eval_layout(long long N, long long S) {
     L.pts_q = o;    o = align_up(o + t * 32, 256);
     L.partial = o;  o = align_up(o + (size_t)blocks_of((long long)t, kChThreads * kSumPer) * 16, 256);
     L.total = o;
+    L.t = t;
     return L;
 }
 
@@ -751,10 +748,6 @@ struct EvalBufs {
     const EvalLayout* L;
     cudaStream_t st;
     unsigned long long* bb() const { return (unsigned long long*)(w + L->ctrl + 64); }
-    uint64_t* ka() const { return (uint64_t*)(w + L->ka); }
-    uint64_t* kb() const { return (uint64_t*)(w + L->kb); }
-    uint32_t* va() const { return (uint32_t*)(w + L->va); }
-    uint32_t* vb() const { return (uint32_t*)(w + L->vb); }
 };
 
 // n points of xyz (n x 3 float64) gathered into Morton order in pts (.w = row); n >= 1
@@ -768,16 +761,16 @@ int sort_points(const EvalBufs& B, uint32_t n, const double* xyz, double4* pts, 
             n, xyz, B.bb());
         SURFEL_CUDA_OK(cudaGetLastError());
     }
+    const RadixSortWs sort = radix_sort_ws(B.w + B.L->sort, B.L->t, 63);
     {
         LaunchScope scope(stage, st);
-        ch_morton_kernel<<<blocks_of(n), kChThreads, 0, st>>>(n, xyz, B.bb(), B.ka(), B.va());
+        ch_morton_kernel<<<blocks_of(n), kChThreads, 0, st>>>(n, xyz, B.bb(), sort.in.keys, sort.in.vals);
         SURFEL_CUDA_OK(cudaGetLastError());
     }
-    if (launch_radix_sort_pairs(B.ka(), B.va(), B.kb(), B.vb(), n, 63, B.w + B.L->temp, st)) return 1;
-    const uint32_t* sorted = (radix_sort_passes(63) & 1) ? B.vb() : B.va();
+    if (launch_radix_sort_pairs(sort, n, st)) return 1;
     {
         LaunchScope scope(stage, st);
-        ch_gather_kernel<<<blocks_of(n), kChThreads, 0, st>>>(n, xyz, sorted, pts);
+        ch_gather_kernel<<<blocks_of(n), kChThreads, 0, st>>>(n, xyz, sort.out.vals, pts);
         SURFEL_CUDA_OK(cudaGetLastError());
     }
     return 0;

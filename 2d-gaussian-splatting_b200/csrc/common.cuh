@@ -80,7 +80,7 @@ struct ImageLayout {
     size_t accum, n_contrib, tile_count, total;  // accum: final_T, M1, M2; n_contrib: last, median; per-tile instance counts
 };
 struct BinningLayout {
-    size_t keys_a, keys_b, vals_a, vals_b, ranges, sort_temp, total;
+    size_t pairs, ranges, temp, total;   // the radix sort's buffers, tile ranges, scratch of either sort
 };
 
 __host__ __device__ inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }

@@ -66,18 +66,25 @@ int launch_duplicate_with_keys(int P, int gx, int gy, int row0, int row1, const 
 int launch_identify_tile_ranges(size_t R, int tiles, const uint64_t* keys_sorted, uint2* ranges,
                                 cudaStream_t stream);
 
-// CUB-free stable LSD radix sort of (u64 key, u32 value) pairs on key bits [0, end_bit).
+// CUB-free stable LSD radix sort of (u64 key, u32 value) pairs on key bits [0, end_bit).  The pairs ping-pong
+// between two buffers, one 8-bit digit per pass; radix_sort_ws() tells the caller which buffer to fill (in) and
+// which one holds the result (out), so no caller needs the pass count.
+constexpr long long kRadixSortMaxPairs = (1ll << 30) - 1;
+struct SortPairs { uint64_t* keys; uint32_t* vals; };
+struct RadixSortWs { SortPairs in, out, spare; void* temp; int end_bit; };   // spare: the buffer that is not out
+int radix_key_bits(unsigned long long max_key);   // least end_bit that orders every key in [0, max_key]
 size_t radix_sort_temp_bytes(size_t n);
-// Data starts in A; buffers ping-pong per 8-bit pass; the sorted result is in B when
-// radix_sort_passes(end_bit) is odd, else in A.
-int radix_sort_passes(int end_bit);
-int launch_radix_sort_pairs(uint64_t* keys_a, uint32_t* vals_a, uint64_t* keys_b,
-                            uint32_t* vals_b, size_t n, int end_bit, void* temp,
-                            cudaStream_t stream);
+size_t radix_sort_pairs_bytes(size_t capacity);       // both buffers for up to `capacity` pairs
+size_t radix_sort_workspace_bytes(size_t capacity);   // both buffers, then the pass scratch
+// Over radix_sort_workspace_bytes(capacity) at base, or over radix_sort_pairs_bytes(capacity) at base when the
+// caller keeps the pass scratch at `temp`; or over buffers A and B that the caller placed itself.
+RadixSortWs radix_sort_ws(void* base, size_t capacity, int end_bit, void* temp = nullptr);
+RadixSortWs radix_sort_ws(SortPairs a, SortPairs b, void* temp, int end_bit);
+int launch_radix_sort_pairs(const RadixSortWs& ws, size_t n, cudaStream_t stream);   // ws.in[0, n) -> ws.out
 
 // Tile-bucketed binning (bucket_sort.cu): counting scatter by tile + per-tile shared-memory sort.
 // Produces ranges + point_list (+ keys_sorted if non-NULL) identical to duplicate -> stable radix
-// sort -> identifyTileRanges.  `pairs` is an R x u64 scratch buffer.
+// sort -> identifyTileRanges.  `pairs` is an R x u64 scratch buffer (the radix sort's spare keys).
 size_t bucket_temp_bytes(int tiles);
 int launch_bucket_binning(int P, size_t R, int gx, int gy, int row0, int row1, const float4* tmat,
                           const int* radii, const uint32_t* offsets, unsigned long long* pairs,

@@ -52,7 +52,7 @@ constexpr int kBox = 32;              // points per level-0 box == lanes per war
 constexpr int kMaxLevels = 8;         // 32^7 boxes of 32 points > 2^30 points
 constexpr int kKnnThreads = 256;
 constexpr uint64_t kNonFiniteKey = 1ull << 63;
-constexpr int kKnnMaxP = (1 << 30) - 1;   // the radix sort's limit; indices fit in u32
+constexpr int kKnnMaxP = (int)kRadixSortMaxPairs;   // indices fit in u32
 
 struct KnnLevels {
     int count;                    // levels allocated for P points (the tree of the n finite ones may be shorter)
@@ -60,7 +60,7 @@ struct KnnLevels {
 };
 
 struct KnnLayout {
-    size_t ctrl, keys_a, keys_b, vals_a, vals_b, sort_temp, pts, boxes, total;
+    size_t ctrl, sort, pts, boxes, total;
     KnnLevels lv;
 };
 
@@ -71,11 +71,7 @@ static KnnLayout knn_layout(int P) {
     const size_t p = P > 0 ? (size_t)P : 1;
     size_t o = 0;
     L.ctrl = o;      o = align_up(o + 64, 256);          // [0..2] lo (ordered u32), [3..5] hi, [6] n finite
-    L.keys_a = o;    o = align_up(o + p * 8, 256);
-    L.keys_b = o;    o = align_up(o + p * 8, 256);
-    L.vals_a = o;    o = align_up(o + p * 4, 256);
-    L.vals_b = o;    o = align_up(o + p * 4, 256);
-    L.sort_temp = o; o = align_up(o + radix_sort_temp_bytes(p), 256);
+    L.sort = o;      o = align_up(o + radix_sort_workspace_bytes(p), 256);
     L.pts = o;       o = align_up(o + p * 16, 256);
     size_t nb = 0, n = ceil_box(p);
     L.lv.count = 0;
@@ -354,8 +350,7 @@ int surfel_knn_mean_sq_dist(int P, const float* xyz, float* out, void* workspace
     cudaStream_t st = (cudaStream_t)stream;
     char* w = (char*)workspace;
     uint32_t* ctrl = (uint32_t*)(w + L.ctrl);
-    uint64_t *ka = (uint64_t*)(w + L.keys_a), *kb = (uint64_t*)(w + L.keys_b);
-    uint32_t *va = (uint32_t*)(w + L.vals_a), *vb = (uint32_t*)(w + L.vals_b);
+    const RadixSortWs sort = radix_sort_ws(w + L.sort, (size_t)P, 64);
     float4* pts = (float4*)(w + L.pts);
     float4* boxes = (float4*)(w + L.boxes);
     const unsigned blocks = (unsigned)((P + kKnnThreads - 1) / kKnnThreads);
@@ -366,12 +361,11 @@ int surfel_knn_mean_sq_dist(int P, const float* xyz, float* out, void* workspace
       knn_bbox_kernel<<<(unsigned)min((size_t)blocks, (size_t)current_device_sm_count() * 8), kKnnThreads, 0, st>>>(P, xyz, ctrl); }
     SURFEL_CUDA_OK(cudaGetLastError());
     { LaunchScope scope(kStKnn, st);
-      knn_morton_kernel<<<blocks, kKnnThreads, 0, st>>>(P, xyz, ctrl, ka, va); }
+      knn_morton_kernel<<<blocks, kKnnThreads, 0, st>>>(P, xyz, ctrl, sort.in.keys, sort.in.vals); }
     SURFEL_CUDA_OK(cudaGetLastError());
-    if (launch_radix_sort_pairs(ka, va, kb, vb, (size_t)P, 64, w + L.sort_temp, st)) return 1;
-    const uint32_t* vals_sorted = (radix_sort_passes(64) & 1) ? vb : va;
+    if (launch_radix_sort_pairs(sort, (size_t)P, st)) return 1;
     { LaunchScope scope(kStKnn, st);
-      knn_gather_kernel<<<blocks, kKnnThreads, 0, st>>>(P, xyz, vals_sorted, pts); }
+      knn_gather_kernel<<<blocks, kKnnThreads, 0, st>>>(P, xyz, sort.out.vals, pts); }
     SURFEL_CUDA_OK(cudaGetLastError());
     // one warp per box; the grids are sized for P points, the kernels read the finite count n
     size_t nboxes = ceil_box((size_t)P);

@@ -260,7 +260,7 @@ CropLayout crop_layout(int side) {
 }
 
 struct MergeLayout {
-    size_t ctrl, status, ka, kb, va, vb, temp, ukeys, total;
+    size_t ctrl, status, sort, ukeys, total;
     int blocks;
 };
 
@@ -271,11 +271,7 @@ MergeLayout merge_layout(long long n) {
     size_t o = 0;
     L.ctrl = o;   o = align_up(o + 64, 256);
     L.status = o; o = align_up(o + (size_t)L.blocks * 8, 256);
-    L.ka = o;     o = align_up(o + m * 8, 256);
-    L.kb = o;     o = align_up(o + m * 8, 256);
-    L.va = o;     o = align_up(o + m * 4, 256);
-    L.vb = o;     o = align_up(o + m * 4, 256);
-    L.temp = o;   o = align_up(o + radix_sort_temp_bytes(m), 256);
+    L.sort = o;   o = align_up(o + radix_sort_workspace_bytes(m), 256);
     L.ukeys = o;  o = align_up(o + m * 8, 256);
     L.total = o;
     return L;
@@ -369,7 +365,7 @@ int surfel_mcubes_crop_emit(int side, const float* volume, const double* bounds,
 }
 
 size_t surfel_mcubes_merge_workspace_bytes(long long n_records) {
-    if (n_records < 0 || n_records >= (1ll << 30)) return 0;
+    if (n_records < 0 || n_records > kRadixSortMaxPairs) return 0;
     return merge_layout(n_records).total;
 }
 
@@ -378,7 +374,7 @@ int surfel_mcubes_merge(long long n_records, const unsigned long long* vert_keys
                         double radius, void* workspace, size_t workspace_bytes, float* verts, long long* faces,
                         long long* n_verts, void* stream) {
     if (n_records < 0 || n_tris < 0) { surfel_set_error("surfel_mcubes_merge: negative count"); return 1; }
-    if (n_records >= (1ll << 30)) {
+    if (n_records > kRadixSortMaxPairs) {
         surfel_set_error("surfel_mcubes_merge: %lld vertex records exceed the radix sort's limit of 2^30", n_records);
         return 1;
     }
@@ -409,21 +405,19 @@ int surfel_mcubes_merge(long long n_records, const unsigned long long* vert_keys
         return 0;
     }
     SURFEL_CUDA_OK(cudaMemsetAsync(w + L.status, 0, (size_t)L.blocks * 8, st));
-    uint64_t *ka = (uint64_t*)(w + L.ka), *kb = (uint64_t*)(w + L.kb);
-    uint32_t *va = (uint32_t*)(w + L.va), *vb = (uint32_t*)(w + L.vb);
+    const RadixSortWs sort = radix_sort_ws(w + L.sort, (size_t)n_records, key_bits);
     const int grid = (int)std::min<long long>((n_records + 255) / 256, (long long)current_device_sm_count() * 8);
     {
         LaunchScope scope(kStMcubesMerge, st);
-        mc_sort_init_kernel<<<grid, 256, 0, st>>>(n_records, vert_keys, ka, va);
+        mc_sort_init_kernel<<<grid, 256, 0, st>>>(n_records, vert_keys, sort.in.keys, sort.in.vals);
         SURFEL_CUDA_OK(cudaGetLastError());
     }
-    if (launch_radix_sort_pairs(ka, va, kb, vb, (size_t)n_records, key_bits, w + L.temp, st)) return 1;
-    const bool in_b = radix_sort_passes(key_bits) & 1;
+    if (launch_radix_sort_pairs(sort, (size_t)n_records, st)) return 1;
     McCtrl m{(uint32_t*)(w + L.ctrl), (unsigned long long*)(w + L.status), nullptr};
     unsigned long long* ukeys = (unsigned long long*)(w + L.ukeys);
     {
         LaunchScope scope(kStMcubesMerge, st);
-        mc_unique_kernel<<<L.blocks, kMcThreads, 0, st>>>(n_records, in_b ? kb : ka, in_b ? vb : va, vert_pos, m,
+        mc_unique_kernel<<<L.blocks, kMcThreads, 0, st>>>(n_records, sort.out.keys, sort.out.vals, vert_pos, m,
                                                            (float)radius, center[0], center[1], center[2], ukeys,
                                                            verts, n_verts);
         SURFEL_CUDA_OK(cudaGetLastError());

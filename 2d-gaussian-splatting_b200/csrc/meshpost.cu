@@ -37,7 +37,7 @@ namespace {
 
 constexpr int kMpThreads = 256;
 constexpr long long kMpMaxVerts = 1ll << 31;      // vertex indices and counts travel in 32 bits
-constexpr long long kMpMaxRecords = 1ll << 30;    // 3 F edge records: the radix sort's limit
+constexpr long long kMpMaxFaces = kRadixSortMaxPairs / 3;   // 3 F edge records go through one radix sort
 constexpr uint32_t kMpMinCluster = 50;            // post_process_mesh's max(n_cluster, 50)
 
 __device__ __forceinline__ uint32_t ld_parent(const uint32_t* p) {
@@ -236,7 +236,7 @@ __global__ void __launch_bounds__(kMpThreads) mp_fscan_kernel(long long F, long 
 int blocks_of(long long n) { return (int)std::max<long long>(1, (n + kMpThreads - 1) / kMpThreads); }
 
 struct MpLayout {
-    size_t ctrl, status_f, status_m, status_c, ka, kb, va, vb, temp, parent, rank, vnew, total;
+    size_t ctrl, status_f, status_m, status_c, sort, parent, rank, vnew, total;
 };
 
 // ctrl: [0..2] tickets of the three scans, [4] error flag
@@ -248,11 +248,7 @@ MpLayout mp_layout(long long M, long long F) {
     L.status_f = o; o = align_up(o + (size_t)blocks_of(F) * 8, 256);
     L.status_m = o; o = align_up(o + (size_t)blocks_of(M) * 8, 256);
     L.status_c = o; o = align_up(o + (size_t)blocks_of(F) * 8, 256);
-    L.ka = o;       o = align_up(o + r * 8, 256);
-    L.kb = o;       o = align_up(o + r * 8, 256);
-    L.va = o;       o = align_up(o + r * 4, 256);
-    L.vb = o;       o = align_up(o + r * 4, 256);
-    L.temp = o;     o = align_up(o + radix_sort_temp_bytes(r), 256);
+    L.sort = o;     o = align_up(o + radix_sort_workspace_bytes(r), 256);
     L.parent = o;   o = align_up(o + f * 4, 256);
     L.rank = o;     o = align_up(o + f * 4, 256);
     L.vnew = o;     o = align_up(o + m * 4, 256);
@@ -266,7 +262,7 @@ bool sizes_ok(const char* who, long long M, long long F) {
         surfel_set_error("%s: %lld vertices; fewer than 2^31 are supported", who, M);
         return false;
     }
-    if (F > (kMpMaxRecords - 1) / 3) {
+    if (F > kMpMaxFaces) {
         surfel_set_error("%s: %lld faces give %lld edge records; the radix sort takes fewer than 2^30", who, F, 3 * F);
         return false;
     }
@@ -282,8 +278,6 @@ bool workspace_ok(const char* who, const void* ws, size_t bytes, const MpLayout&
     return true;
 }
 
-int bit_length(unsigned long long x) { return x ? 64 - __builtin_clzll(x) : 0; }
-
 }  // namespace
 }  // namespace surfel
 
@@ -292,7 +286,7 @@ using namespace surfel;
 extern "C" {
 
 size_t surfel_meshpost_workspace_bytes(long long n_verts, long long n_faces) {
-    if (n_verts < 0 || n_faces < 0 || n_verts >= kMpMaxVerts || n_faces > (kMpMaxRecords - 1) / 3) return 0;
+    if (n_verts < 0 || n_faces < 0 || n_verts >= kMpMaxVerts || n_faces > kMpMaxFaces) return 0;
     return mp_layout(n_verts, n_faces).total;
 }
 
@@ -314,8 +308,8 @@ int surfel_meshpost_clusters(long long n_verts, long long n_faces, const long lo
     }
     char* w = (char*)workspace;
     uint32_t* ctrl = (uint32_t*)(w + L.ctrl);
-    uint64_t *ka = (uint64_t*)(w + L.ka), *kb = (uint64_t*)(w + L.kb);
-    uint32_t *va = (uint32_t*)(w + L.va), *vb = (uint32_t*)(w + L.vb);
+    const unsigned long long M = (unsigned long long)n_verts;
+    const RadixSortWs sort = radix_sort_ws(w + L.sort, 3 * (size_t)n_faces, radix_key_bits(M > 0 ? M * M - 1 : 0));
     uint32_t *parent = (uint32_t*)(w + L.parent), *rank = (uint32_t*)(w + L.rank);
     SURFEL_CUDA_OK(cudaMemsetAsync(ctrl, 0, 64, st));
     SURFEL_CUDA_OK(cudaMemsetAsync(w + L.status_f, 0, (size_t)blocks_of(n_faces) * 8, st));
@@ -323,16 +317,14 @@ int surfel_meshpost_clusters(long long n_verts, long long n_faces, const long lo
     const long long n_rec = 3 * n_faces;
     {
         LaunchScope scope(kStMeshpostEdges, st);
-        mp_edges_kernel<<<blocks_of(n_faces), kMpThreads, 0, st>>>(n_faces, n_verts, faces, ka, va, parent, ctrl + 4);
+        mp_edges_kernel<<<blocks_of(n_faces), kMpThreads, 0, st>>>(n_faces, n_verts, faces, sort.in.keys, sort.in.vals,
+                                                                   parent, ctrl + 4);
         SURFEL_CUDA_OK(cudaGetLastError());
     }
-    const unsigned long long M = (unsigned long long)n_verts;
-    const int key_bits = std::max(1, bit_length(M > 0 ? M * M - 1 : 0));
-    if (launch_radix_sort_pairs(ka, va, kb, vb, (size_t)n_rec, key_bits, w + L.temp, st)) return 1;
-    const bool in_b = radix_sort_passes(key_bits) & 1;
+    if (launch_radix_sort_pairs(sort, (size_t)n_rec, st)) return 1;
     {
         LaunchScope scope(kStMeshpostUnion, st);
-        mp_union_kernel<<<blocks_of(n_rec - 1), kMpThreads, 0, st>>>(n_rec, in_b ? kb : ka, in_b ? vb : va, parent);
+        mp_union_kernel<<<blocks_of(n_rec - 1), kMpThreads, 0, st>>>(n_rec, sort.out.keys, sort.out.vals, parent);
         SURFEL_CUDA_OK(cudaGetLastError());
     }
     {
@@ -377,8 +369,7 @@ int surfel_meshpost_compact(long long n_verts, long long n_faces, const long lon
     cudaStream_t st = (cudaStream_t)stream;
     char* w = (char*)workspace;
     uint32_t* ctrl = (uint32_t*)(w + L.ctrl);
-    uint64_t *ka = (uint64_t*)(w + L.ka), *kb = (uint64_t*)(w + L.kb);
-    uint32_t *va = (uint32_t*)(w + L.va), *vb = (uint32_t*)(w + L.vb);
+    const RadixSortWs sort = radix_sort_ws(w + L.sort, 3 * (size_t)n_faces, radix_key_bits((unsigned long long)n_faces));
     uint32_t* vnew = (uint32_t*)(w + L.vnew);
     SURFEL_CUDA_OK(cudaMemsetAsync(ctrl, 0, 64, st));
     SURFEL_CUDA_OK(cudaMemsetAsync(w + L.status_m, 0, (size_t)blocks_of(n_verts) * 8, st));
@@ -386,12 +377,12 @@ int surfel_meshpost_compact(long long n_verts, long long n_faces, const long lon
     SURFEL_CUDA_OK(cudaMemsetAsync(vnew, 0, (size_t)std::max<long long>(n_verts, 1) * 4, st));
     {
         LaunchScope scope(kStMeshpostCompact, st);
-        mp_count_keys_kernel<<<blocks_of(n_clusters), kMpThreads, 0, st>>>(n_clusters, cluster_count, ka, va);
+        mp_count_keys_kernel<<<blocks_of(n_clusters), kMpThreads, 0, st>>>(n_clusters, cluster_count, sort.in.keys,
+                                                                            sort.in.vals);
         SURFEL_CUDA_OK(cudaGetLastError());
     }
-    const int count_bits = std::max(1, bit_length((unsigned long long)n_faces));
-    if (launch_radix_sort_pairs(ka, va, kb, vb, (size_t)n_clusters, count_bits, w + L.temp, st)) return 1;
-    const uint64_t* kth = (radix_sort_passes(count_bits) & 1 ? kb : ka) + index;
+    if (launch_radix_sort_pairs(sort, (size_t)n_clusters, st)) return 1;
+    const uint64_t* kth = sort.out.keys + index;
     {
         LaunchScope scope(kStMeshpostCompact, st);
         mp_mark_kernel<<<blocks_of(n_faces), kMpThreads, 0, st>>>(n_faces, n_verts, faces, face_cluster, cluster_count,

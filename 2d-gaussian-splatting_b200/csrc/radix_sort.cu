@@ -27,6 +27,7 @@ constexpr int kTile = kSortThreads * kItems;   // 4096 pairs per block
 constexpr int kMaxPasses = 8;
 
 constexpr uint32_t kStAgg = 1u << 30, kStPrefix = 2u << 30, kStMask = (1u << 30) - 1u;
+static_assert(kRadixSortMaxPairs <= kStMask, "a digit's running count must fit the 30 bits of a look-back status word");
 
 struct SortTemp {
     uint32_t* hist;       // [kMaxPasses][kRadix] -> exclusive global digit bases after scan
@@ -235,17 +236,39 @@ radix_onesweep_kernel(const uint64_t* __restrict__ keys_in, const uint32_t* __re
     }
 }
 
-int radix_sort_passes(int end_bit) { return (end_bit + kRadixBits - 1) / kRadixBits; }
+static int radix_sort_passes(int end_bit) { return (end_bit + kRadixBits - 1) / kRadixBits; }
 
-int launch_radix_sort_pairs(uint64_t* keys_a, uint32_t* vals_a, uint64_t* keys_b,
-                            uint32_t* vals_b, size_t n, int end_bit, void* temp,
-                            cudaStream_t stream) {
+int radix_key_bits(unsigned long long max_key) { return max_key ? 64 - __builtin_clzll(max_key) : 1; }
+
+// keys A, keys B, values A, values B
+size_t radix_sort_pairs_bytes(size_t capacity) { return 2 * align_up(capacity * 8, 256) + 2 * align_up(capacity * 4, 256); }
+
+size_t radix_sort_workspace_bytes(size_t capacity) {
+    return radix_sort_pairs_bytes(capacity) + radix_sort_temp_bytes(capacity);
+}
+
+RadixSortWs radix_sort_ws(SortPairs a, SortPairs b, void* temp, int end_bit) {
+    // each pass moves the pairs to the other buffer: after an odd number of passes they are in B
+    const bool in_b = radix_sort_passes(end_bit) & 1;
+    return RadixSortWs{a, in_b ? b : a, in_b ? a : b, temp, end_bit};
+}
+
+RadixSortWs radix_sort_ws(void* base, size_t capacity, int end_bit, void* temp) {
+    char* c = (char*)base;
+    const size_t keys = align_up(capacity * 8, 256), vals = align_up(capacity * 4, 256);
+    const SortPairs a{(uint64_t*)c, (uint32_t*)(c + 2 * keys)};
+    const SortPairs b{(uint64_t*)(c + keys), (uint32_t*)(c + 2 * keys + vals)};
+    return radix_sort_ws(a, b, temp ? temp : c + radix_sort_pairs_bytes(capacity), end_bit);
+}
+
+int launch_radix_sort_pairs(const RadixSortWs& ws, size_t n, cudaStream_t stream) {
     if (n == 0) return 0;
-    if (n >= (1ull << 30)) { surfel_set_error("radix sort: n=%zu exceeds 2^30", n); return 1; }
+    const int end_bit = ws.end_bit;
+    if (n > (size_t)kRadixSortMaxPairs) { surfel_set_error("radix sort: n=%zu exceeds 2^30", n); return 1; }
     if (end_bit < 1 || end_bit > 64) { surfel_set_error("radix sort: bad end_bit %d", end_bit); return 1; }
     const int passes = radix_sort_passes(end_bit);
     const size_t tiles = sort_tiles(n);
-    SortTemp t = carve_temp(temp, n);
+    SortTemp t = carve_temp(ws.temp, n);
     SURFEL_CUDA_OK(cudaMemsetAsync(t.hist, 0, (size_t)kMaxPasses * kRadix * 4, stream));
     SURFEL_CUDA_OK(cudaMemsetAsync(t.tickets, 0, 256, stream));
     SURFEL_CUDA_OK(cudaMemsetAsync(t.status, 0, (size_t)passes * tiles * kRadix * 4, stream));
@@ -260,26 +283,23 @@ int launch_radix_sort_pairs(uint64_t* keys_a, uint32_t* vals_a, uint64_t* keys_b
     }
     const int hist_blocks = (int)std::min((size_t)current_device_sm_count() * 8, (n + 255) / 256);
     { LaunchScope scope(kStSortHist, stream);
-    radix_histogram_kernel<<<hist_blocks, 256, 0, stream>>>(keys_a, n, passes, end_bit, t.hist);
+    radix_histogram_kernel<<<hist_blocks, 256, 0, stream>>>(ws.in.keys, n, passes, end_bit, t.hist);
     SURFEL_CUDA_OK(cudaGetLastError());
     prof_count_launch();
     radix_scan_hist_kernel<<<passes, kRadix, 0, stream>>>(t.hist); }
     SURFEL_CUDA_OK(cudaGetLastError());
 
-    // ping-pong A -> B -> A ...: the result is in B after an odd number of passes, else in A
-    // (radix_sort_passes() tells the caller, who picks its buffers accordingly: no extra copy).
-    uint64_t* ka = keys_a; uint32_t* va = vals_a;
-    uint64_t* kb = keys_b; uint32_t* vb = vals_b;
+    // ping-pong A -> B -> A ...: radix_sort_ws() made `out` the buffer the last pass writes, so no copy follows
+    SortPairs src = ws.in, dst = (passes & 1) ? ws.out : ws.spare;
     for (int ps = 0; ps < passes; ps++) {
         const int shift = ps * kRadixBits;
         const uint32_t mask = (1u << std::min(kRadixBits, end_bit - shift)) - 1u;
         LaunchScope scope(kStSortPass, stream);
         radix_onesweep_kernel<<<(unsigned)tiles, kSortThreads, sizeof(SortSmem), stream>>>(
-            ka, va, kb, vb, n, shift, mask, t.hist + ps * kRadix, t.tickets + ps,
+            src.keys, src.vals, dst.keys, dst.vals, n, shift, mask, t.hist + ps * kRadix, t.tickets + ps,
             t.status + (size_t)ps * tiles * kRadix);
         SURFEL_CUDA_OK(cudaGetLastError());
-        std::swap(ka, kb);
-        std::swap(va, vb);
+        std::swap(src, dst);
     }
     return 0;
 }
