@@ -37,6 +37,7 @@ SOURCES = {
     "meshpost.cu": [],
     "chamfer.cu": ["-fmad=false"],
     "cull.cu": ["-fmad=false"],
+    "metrics.cu": [],
 }
 # Test variants of the library: one render kernel rebuilt with another batch size (slots staged per round), the rest
 # shared with the main library.  tests/test_hitloop_gpu.py runs the whole hit-loop suite against each, so a change

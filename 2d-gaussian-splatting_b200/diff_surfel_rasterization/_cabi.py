@@ -150,6 +150,16 @@ SIGNATURES = {
     "surfel_cull_emit": (c_int, [ctypes.c_longlong, c_void_p, ctypes.c_longlong, c_void_p,
                                  ctypes.POINTER(ctypes.c_double), c_void_p, ctypes.c_longlong, c_void_p, c_size_t,
                                  ctypes.c_longlong, ctypes.c_longlong, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "surfel_metrics_min_side": (c_int, []),
+    "surfel_metrics_max_side": (c_int, []),
+    "surfel_metrics_partials_count": (c_size_t, [c_int]),
+    "surfel_metrics_lpips_input": (c_int, [c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "surfel_metrics_pack_conv": (c_int, [c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "surfel_metrics_conv3x3": (c_int, [c_int, c_int, c_int, c_int, c_int] + [c_void_p] * 5),
+    "surfel_metrics_maxpool": (c_int, [c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "surfel_metrics_lpips_tap": (c_int, [c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "surfel_metrics_lpips_finish": (c_int, [ctypes.POINTER(ctypes.c_longlong)] + [c_void_p] * 4),
+    "surfel_metrics_psnr": (c_int, [c_int, ctypes.c_longlong] + [c_void_p] * 5),
     "surfel_launch_count":(ctypes.c_ulonglong, []),
     "surfel_profile_enable": (None, [c_int]),
     "surfel_profile_num_stages": (c_int, []),

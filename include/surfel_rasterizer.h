@@ -492,6 +492,40 @@ int surfel_cull_emit(long long n_verts, const double* verts, long long n_faces, 
                      size_t workspace_bytes, long long n_kept_verts, long long n_kept_faces, double* out_verts,
                      long long* out_faces, void* out_colors, void* stream);
 
+/* ---- Novel-view metrics (metrics.py of the reference: PSNR of utils/image_utils.py and LPIPS-VGG of lpipsPyTorch;
+ * rules in DESIGN.md §7o, csrc/metrics.cu).  SSIM is surfel_l1_ssim_forward's sums[1] / (C H W).  Activations are
+ * NHWC float32 batches of n images (n = 2 for LPIPS: render then gt).  Each call runs on `stream` and does not
+ * synchronise.
+ *  surfel_metrics_lpips_input: x, y (3 x H x W each, device) z-scored into out (2 x H x W x 3).  Rejects n != 1,
+ *   c != 3, a side outside [surfel_metrics_min_side(), surfel_metrics_max_side()] and host memory.
+ *  surfel_metrics_pack_conv: a conv weight [cout][cin][3][3] to packed [cout][3][3][cin] (rounded to TF32, to
+ *   nearest, when cin % 32 == 0; cin 3 is copied).  cout a multiple of 64.
+ *  surfel_metrics_conv3x3: relu(conv3x3(in, packed, padding 1) + bias), in n x H x W x cin, out n x H x W x cout.
+ *   cin 3 with cout 64 runs in float32; cin % 32 == 0 runs on the TF32 tensor cores (wgmma).
+ *  surfel_metrics_maxpool: 2 x 2 stride-2 max-pool with floor, n x H x W x c to n x (H/2) x (W/2) x c, c % 4 == 0.
+ *  surfel_metrics_lpips_tap: tap (0..4) of the 2 x H x W x c features: the sum over pixels of
+ *   lin . (fx / (|fx| + 1e-10) - fy / (|fy| + 1e-10))^2, as fixed per-block partials in partials (double, at least
+ *   surfel_metrics_partials_count(1) entries).
+ *  surfel_metrics_lpips_finish: out[0] = sum over taps of float32(partial sum / tap_pixels_host[t]); taps (5 floats,
+ *   may be NULL) gets each tap's mean.
+ *  surfel_metrics_psnr: out[i] = float32(20 log10(1 / sqrt(mse_i))), mse of the i-th per_image floats of a and b
+ *   summed in double; partials holds surfel_metrics_partials_count(n) doubles. */
+int surfel_metrics_min_side(void);
+int surfel_metrics_max_side(void);
+size_t surfel_metrics_partials_count(int n_images);
+int surfel_metrics_lpips_input(int n, int c, int height, int width, const float* x, const float* y, float* out,
+                               void* stream);
+int surfel_metrics_pack_conv(int cout, int cin, const float* w, float* packed, void* stream);
+int surfel_metrics_conv3x3(int n, int height, int width, int cin, int cout, const float* in, const float* packed,
+                           const float* bias, float* out, void* stream);
+int surfel_metrics_maxpool(int n, int height, int width, int c, const float* in, float* out, void* stream);
+int surfel_metrics_lpips_tap(int tap, int height, int width, int c, const float* feat, const float* lin,
+                             double* partials, void* stream);
+int surfel_metrics_lpips_finish(const long long* tap_pixels_host, const double* partials, float* out, float* taps,
+                                void* stream);
+int surfel_metrics_psnr(int n, long long per_image, const float* a, const float* b, double* partials, float* out,
+                        void* stream);
+
 /* Instrumentation used by bench.py: number of kernels this library has launched in this process,
  * and optional per-stage CUDA-event timing (events recorded on the launching stream around each
  * kernel while enabled; surfel_profile_read() waits for them and returns summed ms / launch counts
