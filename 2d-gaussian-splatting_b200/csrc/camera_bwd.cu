@@ -1,0 +1,205 @@
+// camera_bwd.cu — gradients of the camera: dL/dviewmatrix, dL/dprojmatrix and dL/dcampos (DESIGN §7p).
+//
+// Runs after surfel_backward on the same stream and workspaces, and reads what that call left behind: the
+// 24-float gradient record (dL_dnormal, dL_dcolor), the full dL_dT after the AABB-centre fold (dL_dtransMat),
+// the stored view-space normal of the render record (its sign is the forward's dual-visible flip) and the clamp
+// bits.  preprocess backward itself is untouched.
+//
+// Per visible splat (row-vector matrices, pr = projmatrix, vm = viewmatrix, 16 contiguous floats each):
+//   G_j[r] = gT[3j] L0[r] + gT[3j+1] L1[r] + gT[3j+2] p[r]  (r < 3),   G_j[3] = gT[3j+2]
+//            L0 = mod s_u R[:,0], L1 = mod s_v R[:,1]  (the forward's T = [L0; L1; p 1] Pm_j, exact in the modifier)
+//   V[r][c] = mult L2[r] gn[c]                               (the stored normal is mult L2 . vm[:3,:3])
+//   C       = -(the SH view-direction term of dL_dmeans3D)   (the direction is means3D - campos)
+// and the finish maps G to projmatrix through ndc2pix:
+//   dpr[4r] = W/2 G_0[r],  dpr[4r+1] = H/2 G_1[r],  dpr[4r+3] = (W-1)/2 G_0[r] + (H-1)/2 G_1[r] + G_2[r],  dpr[4r+2] = 0.
+// On the transMat_precomp path T and the normal do not depend on the camera: only C is formed.
+//
+// Determinism: splat i belongs to block i / chunk for a chunk that depends on P alone; each thread adds its splats'
+// float32 terms into double registers, the block reduces them in a fixed tree into one double partial per term, and
+// one block adds the partials in block order and rounds each output once.  No atomics: repeat calls are
+// bit-identical, on any stream and any device.
+#include <algorithm>
+
+#include "common.cuh"
+#include "kernels.h"
+#include "profile.h"
+
+namespace surfel {
+
+namespace {
+
+__constant__ float k_SH_C2[5] = {1.0925484305920792f, -1.0925484305920792f, 0.31539156525252005f,
+                                 -1.0925484305920792f, 0.5462742152960396f};
+__constant__ float k_SH_C3[7] = {-0.5900435899266435f, 2.890611442640554f, -0.4570457994644658f,
+                                 0.3731763325901154f,  -0.4570457994644658f, 1.445305721320277f,
+                                 -0.5900435899266435f};
+constexpr float kSH_C1 = 0.4886025119029199f;
+
+constexpr int kCamTerms = 24;          // 12 G, 9 V, 3 C
+constexpr int kCamThreads = 256;
+constexpr int kCamMaxBlocks = 1024;
+
+int cam_blocks(int P) { return P <= 0 ? 0 : std::min(kCamMaxBlocks, (P + kCamThreads - 1) / kCamThreads); }
+
+// d(colour . dR)/d(direction) for the unnormalised direction (dx, dy, dz): the SH part of dL_dmeans3D
+__device__ __forceinline__ void sh_direction_grad(const float* __restrict__ sh, int D, const float dR[3], float dx,
+                                                  float dy, float dz, float g[3]) {
+    const float invl = rsqrtf(dx * dx + dy * dy + dz * dz);
+    const float x = dx * invl, y = dy * invl, z = dz * invl;
+    auto dot = [&](int i) { return dR[0] * __ldg(sh + 3 * i) + dR[1] * __ldg(sh + 3 * i + 1) + dR[2] * __ldg(sh + 3 * i + 2); };
+    float gx = 0.0f, gy = 0.0f, gz = 0.0f;
+    if (D > 0) {
+        const float d1 = dot(1), d2 = dot(2), d3 = dot(3);
+        gx += -kSH_C1 * d3; gy += -kSH_C1 * d1; gz += kSH_C1 * d2;
+        if (D > 1) {
+            const float xx = x * x, yy = y * y, zz = z * z, xy = x * y, yz = y * z, xz = x * z;
+            const float d4 = dot(4), d5 = dot(5), d6 = dot(6), d7 = dot(7), d8 = dot(8);
+            gx += k_SH_C2[0] * y * d4 - k_SH_C2[2] * 2.0f * x * d6 + k_SH_C2[3] * z * d7 + k_SH_C2[4] * 2.0f * x * d8;
+            gy += k_SH_C2[0] * x * d4 + k_SH_C2[1] * z * d5 - k_SH_C2[2] * 2.0f * y * d6 - k_SH_C2[4] * 2.0f * y * d8;
+            gz += k_SH_C2[1] * y * d5 + k_SH_C2[2] * 4.0f * z * d6 + k_SH_C2[3] * x * d7;
+            if (D > 2) {
+                const float d9 = dot(9), d10 = dot(10), d11 = dot(11), d12 = dot(12), d13 = dot(13), d14 = dot(14), d15 = dot(15);
+                gx += k_SH_C3[0] * d9 * 6.0f * xy + k_SH_C3[1] * d10 * yz - k_SH_C3[2] * d11 * 2.0f * xy -
+                      k_SH_C3[3] * d12 * 6.0f * xz + k_SH_C3[4] * d13 * (4.0f * zz - 3.0f * xx - yy) +
+                      k_SH_C3[5] * d14 * 2.0f * xz + k_SH_C3[6] * d15 * 3.0f * (xx - yy);
+                gy += k_SH_C3[0] * d9 * 3.0f * (xx - yy) + k_SH_C3[1] * d10 * xz +
+                      k_SH_C3[2] * d11 * (4.0f * zz - xx - 3.0f * yy) - k_SH_C3[3] * d12 * 6.0f * yz -
+                      k_SH_C3[4] * d13 * 2.0f * xy - k_SH_C3[5] * d14 * 2.0f * yz - k_SH_C3[6] * d15 * 6.0f * xy;
+                gz += k_SH_C3[1] * d10 * xy + k_SH_C3[2] * d11 * 8.0f * yz +
+                      k_SH_C3[3] * d12 * 3.0f * (2.0f * zz - xx - yy) + k_SH_C3[4] * d13 * 8.0f * xz +
+                      k_SH_C3[5] * d14 * (xx - yy);
+            }
+        }
+    }
+    // through the normalisation: (I - u u^T) / |d| applied to (gx, gy, gz)
+    const float ug = x * gx + y * gy + z * gz;
+    g[0] = (gx - x * ug) * invl; g[1] = (gy - y * ug) * invl; g[2] = (gz - z * ug) * invl;
+}
+
+}  // namespace
+
+__global__ void __launch_bounds__(kCamThreads) camera_bwd_kernel(CamBwdParams p, int chunk) {
+    double acc[kCamTerms];
+#pragma unroll
+    for (int k = 0; k < kCamTerms; k++) acc[k] = 0.0;
+    const bool geom = p.transMat_precomp == nullptr;
+    const bool has_sh = !p.has_colors_precomp && p.shs != nullptr;
+    const int begin = blockIdx.x * chunk, end = min(p.P, begin + chunk);
+    for (int idx = begin + threadIdx.x; idx < end; idx += kCamThreads) {
+        if (p.radii[idx] <= 0) continue;
+        float t[kCamTerms];
+#pragma unroll
+        for (int k = 0; k < kCamTerms; k++) t[k] = 0.0f;
+        const float px = p.means3D[3 * (size_t)idx], py = p.means3D[3 * (size_t)idx + 1], pz = p.means3D[3 * (size_t)idx + 2];
+        const float4 rg = reinterpret_cast<const float4*>(p.grad_rec + (size_t)idx * kGradFloats)[4];   // gn, gc.x
+        const float2 rg2 = reinterpret_cast<const float2*>(p.grad_rec + (size_t)idx * kGradFloats)[10];  // gc.yz
+        if (geom) {
+            const float4 q = reinterpret_cast<const float4*>(p.rotations)[idx];
+            const float2 sc = reinterpret_cast<const float2*>(p.scales)[idx];
+            const float inv = rsqrtf(q.x * q.x + q.y * q.y + q.z * q.z + q.w * q.w);
+            const float w = q.x * inv, x = q.y * inv, y = q.z * inv, z = q.w * inv;
+            const float su = p.scale_modifier * sc.x, sv = p.scale_modifier * sc.y;
+            const float L0[3] = {(1.0f - 2.0f * (y * y + z * z)) * su, 2.0f * (x * y + w * z) * su, 2.0f * (x * z - w * y) * su};
+            const float L1[3] = {2.0f * (x * y - w * z) * sv, (1.0f - 2.0f * (x * x + z * z)) * sv, 2.0f * (y * z + w * x) * sv};
+            const float L2[3] = {2.0f * (x * z + w * y), 2.0f * (y * z - w * x), 1.0f - 2.0f * (x * x + y * y)};
+            const float pp[3] = {px, py, pz};
+            const float* gT = p.dL_dtransMat + 9 * (size_t)idx;
+#pragma unroll
+            for (int j = 0; j < 3; j++) {
+                const float a = gT[3 * j], b = gT[3 * j + 1], c = gT[3 * j + 2];
+#pragma unroll
+                for (int r = 0; r < 3; r++) t[4 * j + r] = a * L0[r] + b * L1[r] + c * pp[r];
+                t[4 * j + 3] = c;
+            }
+            // the forward stored mult * (L2 . vm[:3,:3]); its sign against the recomputed normal is mult
+            const float4 n = p.rec[(size_t)idx * kRecQuads + 3];
+            const float* vm = p.viewmatrix;
+            const float nv0 = vm[0] * L2[0] + vm[4] * L2[1] + vm[8] * L2[2];
+            const float nv1 = vm[1] * L2[0] + vm[5] * L2[1] + vm[9] * L2[2];
+            const float nv2 = vm[2] * L2[0] + vm[6] * L2[1] + vm[10] * L2[2];
+            const float mult = n.x * nv0 + n.y * nv1 + n.z * nv2 > 0.0f ? 1.0f : -1.0f;
+            const float gn[3] = {rg.x, rg.y, rg.z};
+#pragma unroll
+            for (int r = 0; r < 3; r++) {
+                const float m = mult * L2[r];
+#pragma unroll
+                for (int c = 0; c < 3; c++) t[12 + 3 * r + c] = m * gn[c];
+            }
+        }
+        if (has_sh) {
+            const uint8_t cb = p.clamped[idx];
+            const float dR[3] = {(cb & 1) ? 0.0f : rg.w, (cb & 2) ? 0.0f : rg2.x, (cb & 4) ? 0.0f : rg2.y};
+            if (p.D > 0 && (dR[0] != 0.0f || dR[1] != 0.0f || dR[2] != 0.0f)) {
+                float g[3];
+                sh_direction_grad(p.shs + (size_t)idx * 3 * p.M, p.D, dR, px - p.campos[0], py - p.campos[1],
+                                  pz - p.campos[2], g);
+                t[21] = -g[0]; t[22] = -g[1]; t[23] = -g[2];
+            }
+        }
+#pragma unroll
+        for (int k = 0; k < kCamTerms; k++) acc[k] += (double)t[k];
+    }
+
+    // fixed-order block reduction: warp butterfly, then the warps' sums in warp order
+    __shared__ double s_red[kCamThreads / 32][kCamTerms];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int k = 0; k < kCamTerms; k++) {
+        double v = acc[k];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+        if (lane == 0) s_red[warp][k] = v;
+    }
+    __syncthreads();
+    if (threadIdx.x < kCamTerms) {
+        double s = 0.0;
+#pragma unroll
+        for (int w = 0; w < kCamThreads / 32; w++) s += s_red[w][threadIdx.x];
+        p.partials[(size_t)blockIdx.x * kCamTerms + threadIdx.x] = s;
+    }
+}
+
+__global__ void camera_finish_kernel(int nblocks, int W, int H, const double* __restrict__ partials,
+                                     float* __restrict__ dvm, float* __restrict__ dpr, float* __restrict__ dcam) {
+    __shared__ double s[kCamTerms];
+    const int k = threadIdx.x;
+    if (k < kCamTerms) {
+        double a = 0.0;
+        for (int b = 0; b < nblocks; b++) a += partials[(size_t)b * kCamTerms + k];
+        s[k] = a;
+    }
+    __syncthreads();
+    if (k < 16) {
+        const int r = k >> 2, c = k & 3;
+        const double G0 = s[r], G1 = s[4 + r], G2 = s[8 + r];
+        double v;
+        if (c == 0) v = 0.5 * W * G0;
+        else if (c == 1) v = 0.5 * H * G1;
+        else if (c == 2) v = 0.0;
+        else v = 0.5 * (W - 1) * G0 + 0.5 * (H - 1) * G1 + G2;
+        dpr[k] = (float)v;
+        dvm[k] = (r < 3 && c < 3) ? (float)s[12 + 3 * r + c] : 0.0f;
+    } else if (k < 19) {
+        dcam[k - 16] = (float)s[21 + k - 16];
+    }
+}
+
+size_t camera_partials_bytes(int P) { return (size_t)std::max(1, cam_blocks(P)) * kCamTerms * sizeof(double); }
+
+int launch_camera_bwd(const CamBwdParams& p, cudaStream_t stream) {
+    const int nb = cam_blocks(p.P);
+    if (nb > 0) {
+        const int chunk = (p.P + nb - 1) / nb;
+        LaunchScope scope(kStCameraBwd, stream);
+        camera_bwd_kernel<<<nb, kCamThreads, 0, stream>>>(p, chunk);
+        SURFEL_CUDA_OK(cudaGetLastError());
+    }
+    {
+        LaunchScope scope(kStCameraFinish, stream);
+        camera_finish_kernel<<<1, 32, 0, stream>>>(nb, p.W, p.H, p.partials, p.dL_dviewmatrix, p.dL_dprojmatrix, p.dL_dcampos);
+        SURFEL_CUDA_OK(cudaGetLastError());
+    }
+    return 0;
+}
+
+}  // namespace surfel

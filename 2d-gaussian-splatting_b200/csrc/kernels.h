@@ -37,6 +37,20 @@ struct PreBwdParams {
     int defer_sh;                     // 1: dL_dsh is NOT written; dL_dcolors receives the clamp-masked colour gradient
 };
 
+// camera gradients (camera_bwd.cu): runs after surfel_backward on its record, dL_dT and workspaces
+struct CamBwdParams {
+    int P, D, M, W, H;
+    float scale_modifier;
+    const float* means3D; const float* scales; const float* rotations; const float* shs;
+    const float* transMat_precomp; int has_colors_precomp;
+    const float* viewmatrix; const float* campos;
+    const int* radii; const float4* rec; const uint8_t* clamped;
+    const float* grad_rec;            // (P, kGradFloats) left by surfel_backward
+    const float* dL_dtransMat;        // (P,9) full dL_dT written by preprocess backward (scales+rotations path)
+    double* partials;                 // camera_partials_bytes(P)
+    float* dL_dviewmatrix; float* dL_dprojmatrix; float* dL_dcampos;   // (16), (16), (3) out
+};
+
 struct RenderParams {
     int W, H, gx, gy, row0, row1;
     const uint2* ranges; const uint32_t* point_list; const float4* rec;
@@ -58,6 +72,9 @@ int launch_preprocess_bwd(const PreBwdParams& p, cudaStream_t stream);
 // preprocess_bwd skips in defer_sh mode (so that a multi-GPU caller can reduce 3 floats per splat instead of 3M)
 int launch_sh_grad_expand(int P, int M, int D, const float* means3D, const float* campos,
                           const float* dL_dcolors, float* dL_dsh, cudaStream_t stream);
+
+size_t camera_partials_bytes(int P);
+int launch_camera_bwd(const CamBwdParams& p, cudaStream_t stream);
 
 // binning
 int launch_duplicate_with_keys(int P, int gx, int gy, int row0, int row1, const float4* tmat,

@@ -65,7 +65,8 @@ const char* surfel_profile_stage_name(int stage) {
                                             "mcubes_crop", "mcubes_merge", "meshpost_edges", "meshpost_union",
                                             "meshpost_label", "meshpost_compact", "chamfer_sample",
                                             "chamfer_downsample", "chamfer_select", "chamfer_nn", "cull_dilate",
-                                            "cull_vertices", "cull_faces", "cull_emit"};
+                                            "cull_vertices", "cull_faces", "cull_emit", "camera_bwd",
+                                            "camera_finish"};
     return stage >= 0 && stage < kNumStages ? names[stage] : "";
 }
 int surfel_profile_read(double* ms_out, int* count_out) {

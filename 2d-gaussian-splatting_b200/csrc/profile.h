@@ -10,7 +10,7 @@ enum Stage { kStPreFwd = 0, kStDuplicate, kStSortHist, kStSortPass, kStRanges, k
              kStTileSort, kStAdam, kStDensifyStats, kStPlyUnpack, kStPlyPack, kStKnn, kStDensify, kStTsdf, kStMcubesCrop,
              kStMcubesMerge, kStMeshpostEdges, kStMeshpostUnion, kStMeshpostLabel, kStMeshpostCompact,
              kStChamferSample, kStChamferDownsample, kStChamferSelect, kStChamferNn,
-             kStCullDilate, kStCullVertices, kStCullFaces, kStCullEmit, kNumStages };
+             kStCullDilate, kStCullVertices, kStCullFaces, kStCullEmit, kStCameraBwd, kStCameraFinish, kNumStages };
 
 void prof_count_launch();
 bool prof_enabled();

@@ -304,62 +304,122 @@ class _RasterizeGaussians(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, grad_color, grad_radii, grad_allmap):
-        _mark("bwd_enter")
-        lib = _cabi.load()
-        rs = ctx.raster_settings
-        means3D, scales, rotations, cov3Ds, sh, radii, geom, binning, img = ctx.saved_tensors
-        has_sh, has_colors, has_scales, has_cov = ctx.flags
-        P, M, R = means3D.shape[0], ctx.M, ctx.num_rendered
-        dev = means3D.device
-        H, W = int(rs.image_height), int(rs.image_width)
-        keep = []
-        if grad_color is None:
-            grad_color = torch.zeros((3, H, W), device=dev)
-        if grad_allmap is None:
-            grad_allmap = torch.zeros((7, H, W), device=dev)
-        # cotangents are read in place when they are plane-strided views with contiguous rows (e.g. slices of a
-        # padded frame); anything else is made contiguous first
-        gp = _plane_stride(grad_color, 3, H, W)
-        if gp is None or _plane_stride(grad_allmap, 7, H, W) != gp:
-            gp = 0
-            g_color, g_all = _dev_f32(grad_color, "grad_color"), _dev_f32(grad_allmap, "grad_allmap")
-        else:
-            g_color, g_all = grad_color, grad_allmap
-        b = getattr(ctx, "bwd_bufs", None)
-        if b is None:      # P == 0, or backward called twice (retain_graph): allocate here
-            b = _grad_buffers(lib, dev, P, M, has_sh, has_colors, has_scales, has_cov, defer_sh=getattr(ctx, "defer_sh", False))
-        ctx.bwd_bufs = None
-        ctx.grad_bucket = b["bucket"]
-        defer = b["defer_sh"]
-        cs = _settings_struct(rs, keep, out_plane=getattr(ctx, "out_plane", 0), grad_plane=gp, defer_sh=defer)
-        # deferred SH gradient: the caller (surfel_parallel._BandFrame) reduces the bucket and then calls expand()
-        ctx.sh_expand = None
-        if defer:
-            d_col_t, d_sh_t, campos_t = b["d_colors"], b["d_sh"], keep[3]
+        grads, _ = _backward(ctx, grad_color, grad_allmap, camera=False)
+        return grads + (None,)
 
-            def expand():
-                with torch.cuda.device(dev):
-                    _cabi.check(lib.surfel_sh_grad_expand(P, M, int(rs.sh_degree), means3D.data_ptr(), campos_t.data_ptr(),
-                                                          d_col_t.data_ptr(), d_sh_t.data_ptr(),
-                                                          torch.cuda.current_stream(dev).cuda_stream))
-            ctx.sh_expand = expand
-        d_means2D, d_opacity, d_means3D = b["d_means2D"], b["d_opacity"], b["d_means3D"]
-        d_colors, d_cov, d_sh, d_scales, d_rot, scratch = b["d_colors"], b["d_cov"], b["d_sh"], b["d_scales"], b["d_rot"], b["scratch"]
-        stream = torch.cuda.current_stream(dev).cuda_stream
-        with torch.cuda.device(dev):
-            _cabi.check(lib.surfel_backward(
-                ctypes.byref(cs), P, M, R, _ptr(means3D), _ptr(scales), _ptr(rotations), _ptr(cov3Ds),
-                _ptr(sh), int(has_colors), radii.data_ptr(), geom.data_ptr(), binning.data_ptr(),
-                img.data_ptr(), g_color.data_ptr(), g_all.data_ptr(), scratch.data_ptr(),
-                d_means2D.data_ptr(), _ptr(d_colors), d_opacity.data_ptr(), d_means3D.data_ptr(),
-                _ptr(d_cov), _ptr(d_sh), _ptr(d_scales), _ptr(d_rot), int(LOWPASS_DEPTH_QUIRK), stream))
-        _mark("bwd_launched")
-        # (means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, settings)
-        return d_means3D, d_means2D, d_sh, (d_colors if has_colors else None), d_opacity, d_scales, d_rot, d_cov, None
+
+def _backward(ctx, grad_color, grad_allmap, camera):
+    """The backward of both autograd nodes: the eight splat gradients in the order of the node's splat inputs, and,
+    when `camera` is set, (dL_dviewmatrix (16), dL_dprojmatrix (16), dL_dcampos (3)) from surfel_camera_backward."""
+    _mark("bwd_enter")
+    lib = _cabi.load()
+    rs = ctx.raster_settings
+    means3D, scales, rotations, cov3Ds, sh, radii, geom, binning, img = ctx.saved_tensors
+    has_sh, has_colors, has_scales, has_cov = ctx.flags
+    P, M, R = means3D.shape[0], ctx.M, ctx.num_rendered
+    dev = means3D.device
+    H, W = int(rs.image_height), int(rs.image_width)
+    keep = []
+    if grad_color is None:
+        grad_color = torch.zeros((3, H, W), device=dev)
+    if grad_allmap is None:
+        grad_allmap = torch.zeros((7, H, W), device=dev)
+    # cotangents are read in place when they are plane-strided views with contiguous rows (e.g. slices of a
+    # padded frame); anything else is made contiguous first
+    gp = _plane_stride(grad_color, 3, H, W)
+    if gp is None or _plane_stride(grad_allmap, 7, H, W) != gp:
+        gp = 0
+        g_color, g_all = _dev_f32(grad_color, "grad_color"), _dev_f32(grad_allmap, "grad_allmap")
+    else:
+        g_color, g_all = grad_color, grad_allmap
+    b = getattr(ctx, "bwd_bufs", None)
+    if b is None:      # P == 0, or backward called twice (retain_graph): allocate here
+        b = _grad_buffers(lib, dev, P, M, has_sh, has_colors, has_scales, has_cov, defer_sh=getattr(ctx, "defer_sh", False))
+    ctx.bwd_bufs = None
+    ctx.grad_bucket = b["bucket"]
+    defer = b["defer_sh"]
+    cs = _settings_struct(rs, keep, out_plane=getattr(ctx, "out_plane", 0), grad_plane=gp, defer_sh=defer)
+    # deferred SH gradient: the caller (surfel_parallel._BandFrame) reduces the bucket and then calls expand()
+    ctx.sh_expand = None
+    if defer:
+        d_col_t, d_sh_t, campos_t = b["d_colors"], b["d_sh"], keep[3]
+
+        def expand():
+            with torch.cuda.device(dev):
+                _cabi.check(lib.surfel_sh_grad_expand(P, M, int(rs.sh_degree), means3D.data_ptr(), campos_t.data_ptr(),
+                                                      d_col_t.data_ptr(), d_sh_t.data_ptr(),
+                                                      torch.cuda.current_stream(dev).cuda_stream))
+        ctx.sh_expand = expand
+    d_means2D, d_opacity, d_means3D = b["d_means2D"], b["d_opacity"], b["d_means3D"]
+    d_colors, d_cov, d_sh, d_scales, d_rot, scratch = b["d_colors"], b["d_cov"], b["d_sh"], b["d_scales"], b["d_rot"], b["scratch"]
+    stream = torch.cuda.current_stream(dev).cuda_stream
+    # the camera gradient needs the full dL_dT that preprocess backward forms anyway: on the scales+rotations path it
+    # is requested into a buffer of its own (with transMat_precomp it is d_cov, and the camera step does not read it)
+    d_tmat = d_cov
+    if camera and d_tmat is None and has_scales:
+        d_tmat = torch.empty((P, 9), dtype=torch.float32, device=dev)
+    cam = None
+    with torch.cuda.device(dev):
+        _cabi.check(lib.surfel_backward(
+            ctypes.byref(cs), P, M, R, _ptr(means3D), _ptr(scales), _ptr(rotations), _ptr(cov3Ds),
+            _ptr(sh), int(has_colors), radii.data_ptr(), geom.data_ptr(), binning.data_ptr(),
+            img.data_ptr(), g_color.data_ptr(), g_all.data_ptr(), scratch.data_ptr(),
+            d_means2D.data_ptr(), _ptr(d_colors), d_opacity.data_ptr(), d_means3D.data_ptr(),
+            _ptr(d_tmat), _ptr(d_sh), _ptr(d_scales), _ptr(d_rot), int(LOWPASS_DEPTH_QUIRK), stream))
+        if camera:
+            partials = torch.empty((lib.surfel_camera_partials_bytes(P) // 8,), dtype=torch.float64, device=dev)
+            out = torch.empty((35,), dtype=torch.float32, device=dev)
+            _cabi.check(lib.surfel_camera_backward(
+                ctypes.byref(cs), P, M, _ptr(means3D), _ptr(scales), _ptr(rotations), _ptr(cov3Ds), _ptr(sh),
+                int(has_colors), radii.data_ptr(), geom.data_ptr(), scratch.data_ptr(), _ptr(d_tmat),
+                partials.data_ptr(), out[0:16].data_ptr(), out[16:32].data_ptr(), out[32:35].data_ptr(), stream))
+            cam = (out[0:16], out[16:32], out[32:35])
+    _mark("bwd_launched")
+    # (means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp)
+    return (d_means3D, d_means2D, d_sh, (d_colors if has_colors else None), d_opacity, d_scales, d_rot, d_cov), cam
+
+
+class _RasterizeGaussiansCamera(torch.autograd.Function):
+    """The same op with the camera as three more differentiable inputs: viewmatrix (4,4), projmatrix (4,4) and campos
+    (3), in the row-vector layout of GaussianRasterizationSettings.  rasterize_gaussians routes here only when one of
+    them requires grad; the splat gradients are those of _RasterizeGaussians, the camera gradients come from
+    surfel_camera_backward (DESIGN.md §7p).  The whole frame only: a tile-row band would give per-rank partial sums."""
+
+    @staticmethod
+    def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
+                viewmatrix, projmatrix, campos, raster_settings):
+        rs = raster_settings
+        if any(getattr(rs, k, None) is not None for k in ("tile_rows", "out_buffers", "out_replicas")):
+            raise RuntimeError("diff_surfel_rasterization: camera gradients are not available with tile_rows, "
+                               "out_buffers or out_replicas (a tile-row band holds only part of the frame)")
+        ctx.cam_meta = tuple((t.shape, t.dtype) for t in (viewmatrix, projmatrix, campos))
+        rs = rs._replace(viewmatrix=viewmatrix, projmatrix=projmatrix, campos=campos)
+        return _RasterizeGaussians.forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
+                                           cov3Ds_precomp, rs)
+
+    @staticmethod
+    def backward(ctx, grad_color, grad_radii, grad_allmap):
+        grads, cam = _backward(ctx, grad_color, grad_allmap, camera=True)
+        cam = tuple(g.reshape(shape).to(dtype) for g, (shape, dtype) in zip(cam, ctx.cam_meta))
+        return grads + cam + (None,)
+
+
+def _wants_camera_grad(rs):
+    return torch.is_grad_enabled() and any(
+        torch.is_tensor(t) and t.requires_grad for t in (rs.viewmatrix, rs.projmatrix, rs.campos))
+
+
 
 
 def rasterize_gaussians(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
                         cov3Ds_precomp, raster_settings):
+    """The op.  When grad mode is on and raster_settings.viewmatrix, projmatrix or campos requires grad, the
+    rasterizer also differentiates in the camera (_RasterizeGaussiansCamera); otherwise the camera is a constant, as
+    upstream treats it."""
+    if _wants_camera_grad(raster_settings):
+        rs = raster_settings
+        return _RasterizeGaussiansCamera.apply(means3D, means2D, sh, colors_precomp, opacities, scales, rotations,
+                                               cov3Ds_precomp, rs.viewmatrix, rs.projmatrix, rs.campos, rs)
     return _RasterizeGaussians.apply(means3D, means2D, sh, colors_precomp, opacities, scales,
                                      rotations, cov3Ds_precomp, raster_settings)
 

@@ -13,6 +13,9 @@ that wants the fused path replaces lines :118-147 of its render() by
 `surface_regularizers(allmap, camera, depth_ratio, lambda_normal, lambda_dist)` goes from `allmap`
 straight to the two regularisers of the reference's train.py (normal consistency and depth distortion),
 two kernels each way with no intermediate plane (see its docstring).
+
+Both treat the camera as a constant: they return no gradient for world_view_transform or full_proj_transform.  A
+caller that refines the camera through the rasterizer (DESIGN.md §7p) keeps the reference's torch tail, which does.
 """
 import torch
 

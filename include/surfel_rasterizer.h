@@ -173,6 +173,24 @@ int surfel_backward(const surfel_settings_t* s, int P, int M, uint32_t R, const 
                     float* dL_dtransMat, float* dL_dsh, float* dL_dscales, float* dL_drotations,
                     int lowpass_depth_quirk, void* stream);
 
+/* Camera gradients (DESIGN.md §7p): dL_dviewmatrix (16), dL_dprojmatrix (16) and dL_dcampos (3), in the layout of
+ * surfel_settings.viewmatrix / projmatrix / campos (row-vector matrices, 16 contiguous floats).  Call it after
+ * surfel_backward, on the same stream, with the same settings, inputs and geometry workspace.  It reads:
+ *   grad_scratch   the gradient record surfel_backward left there (normal and colour gradients);
+ *   dL_dtransMat   (P,9) the dL_dtransMat surfel_backward wrote: required on the scales+rotations path (pass a
+ *                  buffer to surfel_backward there), ignored with transMat_precomp;
+ *   geom_ws        the stored normals (their sign is the forward's dual-visible flip) and the clamp bits;
+ *   radii, means3D, scales, rotations, shs (SH view direction), settings.campos and settings.viewmatrix.
+ * Only splats with radii > 0 contribute.  With transMat_precomp only dL_dcampos can be non-zero; with colors_precomp
+ * (or sh_degree 0) dL_dcampos is zero.  partials: surfel_camera_partials_bytes(P) bytes of scratch.  There are no
+ * atomics: a repeat call on the same inputs gives bit-identical outputs.  A tile-row band is rejected. */
+size_t surfel_camera_partials_bytes(int P);
+int surfel_camera_backward(const surfel_settings_t* s, int P, int M, const float* means3D, const float* scales,
+                           const float* rotations, const float* transMat_precomp, const float* shs,
+                           int has_colors_precomp, const int32_t* radii, const void* geom_ws,
+                           const float* grad_scratch, const float* dL_dtransMat, double* partials,
+                           float* dL_dviewmatrix, float* dL_dprojmatrix, float* dL_dcampos, void* stream);
+
 /* dL_dsh (P,M,3) = basis_k(normalize(means3D - campos)) * dL_dcolors[c] for k < (sh_degree+1)^2, zero beyond:
  * the expansion surfel_backward() skips when surfel_settings.sh_grad_deferred = 1.  Rows of splats whose
  * colour gradient is exactly zero are zero. */
