@@ -118,21 +118,28 @@ __global__ void post_bwd_normal_vjp_kernel(int W, int H, const float* __restrict
     for (int k = 0; k < 6; k++) tmp[k * N + i] = o[k];
 }
 
-// gather the point gradients (tmp) of the 4 neighbours, chain them with g_depth (the cotangent of surf_depth) to
-// depth and write allmap channels 0, 1 and 5
-__device__ __forceinline__ void depth_chain(int W, int H, int x, int y, float ratio, const float* __restrict__ allmap,
-                                            const float* __restrict__ rays, const float* __restrict__ tmp,
-                                            float g_depth, float* __restrict__ g_allmap) {
+// the gradient of the point P[y,x]: the point gradients (tmp) of its 4 neighbours' stencils
+__device__ __forceinline__ void gather_dP(int W, int H, int x, int y, const float* __restrict__ tmp, float dP[3]) {
     const int N = W * H, i = y * W + x;
     // P[y,x] is "P[y+1]" of pixel (y-1,x), "P[y-1]" of (y+1,x), "P[x+1]" of (y,x-1), "P[x-1]" of (y,x+1)
-    float dP[3] = {0, 0, 0};
 #pragma unroll
     for (int k = 0; k < 3; k++) {
+        dP[k] = 0.0f;
         if (y > 0) dP[k] += tmp[k * N + i - W];
         if (y < H - 1) dP[k] -= tmp[k * N + i + W];
         if (x > 0) dP[k] += tmp[(3 + k) * N + i - 1];
         if (x < W - 1) dP[k] -= tmp[(3 + k) * N + i + 1];
     }
+}
+
+// chain the point gradient (gathered from tmp) with g_depth (the cotangent of surf_depth) to depth and write allmap
+// channels 0, 1 and 5
+__device__ __forceinline__ void depth_chain(int W, int H, int x, int y, float ratio, const float* __restrict__ allmap,
+                                            const float* __restrict__ rays, const float* __restrict__ tmp,
+                                            float g_depth, float* __restrict__ g_allmap) {
+    const int N = W * H, i = y * W + x;
+    float dP[3];
+    gather_dP(W, H, x, y, tmp, dP);
     const float fx = (float)x, fy = (float)y;
     const float r0 = fx * rays[0] + fy * rays[3] + rays[6], r1 = fx * rays[1] + fy * rays[4] + rays[7],
                 r2 = fx * rays[2] + fy * rays[5] + rays[8];
@@ -296,6 +303,108 @@ __global__ void post_reg_bwd_allmap_kernel(int W, int H, float ratio, const floa
     g_allmap[6 * N + i] = gscale[1];
 }
 
+// ---- camera gradients of the tail (DESIGN §7q): dL/drot (9) and dL/drays (12), after either backward above -------
+//   G_rot[3r+c]  = sum_p n_view_r(p) gw_c(p)           gw: the cotangent of rend_normal (world space)
+//   G_rays[3k+j] = sum_p d(p) q_k(p) dP_j(p)           q = (x, y, 1), d = surf_depth, dP the point gradient
+//   G_rays[9+j]  = sum_p dP_j(p)
+// Each thread forms its pixels' 21 float32 terms and adds them into double registers; the block reduces them in a
+// fixed tree into one double partial per term, and one block adds the partials in a fixed order and rounds each
+// output once.  No atomics: repeat calls are bit-identical, on any stream.
+constexpr int kCamTerms = 21;       // 9 rot, 12 rays
+constexpr int kCamRows = 8;         // rows per thread: a 32x8 block covers 32 x 64 pixels
+
+// kReg: the regularisers' backward (gw = -gscale[0] sn, sn formed from allmap as post_reg_bwd_normal_kernel does,
+// d = surf_depth_at); otherwise surface_outputs' (gw = g_rend_normal, may be NULL; d = the saved surf_depth).
+// tmp NULL: no point gradient (G_rays = 0).  partials: term-major, partials[k * nblocks + block].
+template <bool kReg>
+__global__ void __launch_bounds__(kRegThreads)
+post_camera_kernel(int W, int H, float ratio, const float* __restrict__ allmap, const float* __restrict__ rays,
+                   const float* __restrict__ surf_depth, const float* __restrict__ g_rend_normal,
+                   const float* __restrict__ gscale, const float* __restrict__ tmp, double* __restrict__ partials) {
+    double acc[kCamTerms];
+#pragma unroll
+    for (int k = 0; k < kCamTerms; k++) acc[k] = 0.0;
+    const int N = W * H;
+    const int x = blockIdx.x * blockDim.x + threadIdx.x;
+    const bool with_rot = kReg || g_rend_normal != nullptr;
+    const float s = kReg ? gscale[0] : 0.0f;
+    if (x < W) {
+        for (int r = 0; r < kCamRows; r++) {
+            const int y = (blockIdx.y * kCamRows + r) * blockDim.y + threadIdx.y;
+            if (y >= H) break;
+            const int i = y * W + x;
+            if (with_rot) {
+                float gw[3] = {0, 0, 0};
+                if (kReg) {
+                    if (x > 0 && y > 0 && x < W - 1 && y < H - 1) {
+                        float dx[3], dy[3];
+                        stencil_from_allmap(W, x, y, ratio, allmap, rays, N, dx, dy);
+                        const float v0 = dx[1] * dy[2] - dx[2] * dy[1], v1 = dx[2] * dy[0] - dx[0] * dy[2],
+                                    v2 = dx[0] * dy[1] - dx[1] * dy[0];
+                        const float inv = 1.0f / fmaxf(sqrtf(v0 * v0 + v1 * v1 + v2 * v2), 1e-12f);
+                        const float al = allmap[N + i];
+                        gw[0] = -s * (v0 * inv * al); gw[1] = -s * (v1 * inv * al); gw[2] = -s * (v2 * inv * al);
+                    }
+                } else {
+                    gw[0] = g_rend_normal[i]; gw[1] = g_rend_normal[N + i]; gw[2] = g_rend_normal[2 * N + i];
+                }
+                const float nv[3] = {allmap[2 * N + i], allmap[3 * N + i], allmap[4 * N + i]};
+#pragma unroll
+                for (int a = 0; a < 3; a++)
+#pragma unroll
+                    for (int c = 0; c < 3; c++) acc[3 * a + c] += (double)(nv[a] * gw[c]);
+            }
+            if (tmp) {
+                float dP[3];
+                gather_dP(W, H, x, y, tmp, dP);
+                const float d = kReg ? surf_depth_at(allmap, N, i, ratio) : surf_depth[i];
+                const float dq[3] = {d * (float)x, d * (float)y, d};
+#pragma unroll
+                for (int k = 0; k < 3; k++)
+#pragma unroll
+                    for (int j = 0; j < 3; j++) acc[9 + 3 * k + j] += (double)(dq[k] * dP[j]);
+#pragma unroll
+                for (int j = 0; j < 3; j++) acc[18 + j] += (double)dP[j];
+            }
+        }
+    }
+
+    // fixed-order block reduction: warp butterfly, then the warps' sums in warp order
+    __shared__ double s_red[kRegThreads / 32][kCamTerms];
+    const int tid = threadIdx.y * blockDim.x + threadIdx.x, lane = tid & 31, warp = tid >> 5;
+#pragma unroll
+    for (int k = 0; k < kCamTerms; k++) {
+        double v = acc[k];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+        if (lane == 0) s_red[warp][k] = v;
+    }
+    __syncthreads();
+    if (tid < kCamTerms) {
+        double a = 0.0;
+#pragma unroll
+        for (int w = 0; w < kRegThreads / 32; w++) a += s_red[w][tid];
+        const int nblocks = gridDim.x * gridDim.y;
+        partials[(size_t)tid * nblocks + blockIdx.y * gridDim.x + blockIdx.x] = a;
+    }
+}
+
+// one block, one warp per term: lane l adds the partials l, l + 32, ... in order, then a warp butterfly; each output
+// is rounded to float32 once
+__global__ void __launch_bounds__(32 * kCamTerms)
+post_camera_finish_kernel(int nblocks, const double* __restrict__ partials, float* __restrict__ g_rot9,
+                          float* __restrict__ g_rays12) {
+    const int k = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    double a = 0.0;
+    for (int b = lane; b < nblocks; b += 32) a += partials[(size_t)k * nblocks + b];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
+    if (lane == 0) {
+        if (k < 9) g_rot9[k] = (float)a;
+        else g_rays12[k - 9] = (float)a;
+    }
+}
+
 }  // namespace surfel
 
 using namespace surfel;
@@ -400,6 +509,66 @@ int surfel_post_reg_backward(int W, int H, float depth_ratio, double lambda_norm
                                                     gscale2, g_allmap);
     SURFEL_CUDA_OK(cudaGetLastError());
     return 0;
+}
+
+static dim3 post_camera_grid(int W, int H) { return dim3((W + 31) / 32, (H + 8 * kCamRows - 1) / (8 * kCamRows)); }
+
+size_t surfel_post_camera_partials_bytes(int W, int H) {
+    if (!post_size_ok(W, H)) return 0;
+    const dim3 g = post_camera_grid(W, H);
+    return (size_t)kCamTerms * sizeof(double) * g.x * g.y;
+}
+
+// the camera pass and its finish on the stream of the backward it follows
+static int launch_post_camera(bool reg, int W, int H, float ratio, const float* allmap, const float* rays,
+                              const float* surf_depth, const float* g_rend_normal, const float* gscale,
+                              const float* tmp, double* partials, float* g_rot9, float* g_rays12, cudaStream_t st) {
+    const dim3 blk(32, 8), grd = post_camera_grid(W, H);
+    prof_count_launch(); prof_count_launch();
+    if (reg) {
+        post_camera_kernel<true><<<grd, blk, 0, st>>>(W, H, ratio, allmap, rays, nullptr, nullptr, gscale, tmp, partials);
+    } else {
+        post_camera_kernel<false><<<grd, blk, 0, st>>>(W, H, ratio, allmap, rays, surf_depth, g_rend_normal, nullptr,
+                                                       tmp, partials);
+    }
+    SURFEL_CUDA_OK(cudaGetLastError());
+    post_camera_finish_kernel<<<1, 32 * kCamTerms, 0, st>>>(grd.x * grd.y, partials, g_rot9, g_rays12);
+    SURFEL_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
+int surfel_post_camera_backward(int W, int H, float depth_ratio, const float* allmap, const float* rot,
+                                const float* rays, const float* surf_depth, const float* g_rend_normal,
+                                const float* g_surf_depth, const float* g_surf_normal, const float* tmp6,
+                                double* partials, float* g_rot9, float* g_rays12, void* stream) {
+    (void)g_surf_depth;                                       // surf_depth's cotangent does not reach the camera
+    if (!post_size_ok(W, H)) { surfel_set_error("surfel_post_camera_backward: bad size"); return 1; }
+    if (!allmap || !rot || !rays || !surf_depth || !tmp6 || !partials || !g_rot9 || !g_rays12) {
+        surfel_set_error("surfel_post_camera_backward: NULL required pointer"); return 1;
+    }
+    // without g_surf_normal the backward left tmp6 zero: no point gradient to read
+    return launch_post_camera(false, W, H, depth_ratio, allmap, rays, surf_depth, g_rend_normal, nullptr,
+                              g_surf_normal ? tmp6 : nullptr, partials, g_rot9, g_rays12, (cudaStream_t)stream);
+}
+
+int surfel_post_reg_camera_backward(int W, int H, float depth_ratio, double lambda_normal, double lambda_dist,
+                                    const float* allmap, const float* rot, const float* rays, const float* gscale2,
+                                    const float* tmp6, double* partials, float* g_rot9, float* g_rays12,
+                                    void* stream) {
+    (void)lambda_dist;                                        // rend_dist does not depend on the camera
+    if (!post_size_ok(W, H)) { surfel_set_error("surfel_post_reg_camera_backward: bad size"); return 1; }
+    const bool with_normal = lambda_normal != 0.0;
+    if (!allmap || !rot || !rays || !gscale2 || !g_rot9 || !g_rays12 || (with_normal && (!tmp6 || !partials))) {
+        surfel_set_error("surfel_post_reg_camera_backward: NULL required pointer"); return 1;
+    }
+    cudaStream_t st = (cudaStream_t)stream;
+    if (!with_normal) {                                       // only the normal term depends on the camera
+        SURFEL_CUDA_OK(cudaMemsetAsync(g_rot9, 0, 9 * sizeof(float), st));
+        SURFEL_CUDA_OK(cudaMemsetAsync(g_rays12, 0, 12 * sizeof(float), st));
+        return 0;
+    }
+    return launch_post_camera(true, W, H, depth_ratio, allmap, rays, nullptr, nullptr, gscale2, tmp6, partials, g_rot9,
+                              g_rays12, st);
 }
 
 }  // extern "C"

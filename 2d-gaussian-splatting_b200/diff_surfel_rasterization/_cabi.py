@@ -89,6 +89,10 @@ SIGNATURES = {
                                 + [c_void_p]),
     "surfel_post_reg_backward": (c_int, [c_int, c_int, c_float, ctypes.c_double, ctypes.c_double] + [c_void_p] * 6
                                  + [c_void_p]),
+    "surfel_post_camera_partials_bytes": (c_size_t, [c_int, c_int]),
+    "surfel_post_camera_backward": (c_int, [c_int, c_int, c_float] + [c_void_p] * 11 + [c_void_p]),
+    "surfel_post_reg_camera_backward": (c_int, [c_int, c_int, c_float, ctypes.c_double, ctypes.c_double]
+                                        + [c_void_p] * 8 + [c_void_p]),
     "surfel_l1_ssim_forward": (c_int, [c_int, c_int, c_int] + [c_void_p] * 6 + [c_void_p]),
     "surfel_l1_ssim_backward": (c_int, [c_int, c_int, c_int] + [c_void_p] * 7 + [c_void_p]),
     "surfel_adam_step": (c_int, [c_int, ctypes.POINTER(AdamGroup), ctypes.c_double, ctypes.c_double, ctypes.c_double, c_void_p]),

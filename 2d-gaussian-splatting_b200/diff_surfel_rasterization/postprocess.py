@@ -14,8 +14,11 @@ that wants the fused path replaces lines :118-147 of its render() by
 straight to the two regularisers of the reference's train.py (normal consistency and depth distortion),
 two kernels each way with no intermediate plane (see its docstring).
 
-Both treat the camera as a constant: they return no gradient for world_view_transform or full_proj_transform.  A
-caller that refines the camera through the rasterizer (DESIGN.md §7p) keeps the reference's torch tail, which does.
+Both are differentiable in the camera, as the reference's tail is: when world_view_transform or
+full_proj_transform requires grad, the backward adds one more pass (csrc/postprocess.cu, DESIGN.md §7q) that sums
+dL/drot and dL/drays over the frame, and torch autograd carries them through _view_matrices to the two matrices.
+A caller that refines the pose through the rasterizer (DESIGN.md §7p) can keep the fused tail.  Without camera
+gradients the backward runs the same launches as before.
 """
 import torch
 
@@ -35,6 +38,12 @@ def _view_matrices(world_view_transform, full_proj_transform, W, H):
     rays = torch.cat([M.reshape(-1), c2w[:3, 3]]).contiguous()
     rot = wvt[:3, :3].T.contiguous()
     return rot, rays
+
+
+def _camera_buffers(lib, W, H, dev):
+    """Scratch and outputs of the camera pass: partials, dL/drot (3,3) and dL/drays (12,)."""
+    partials = torch.empty(lib.surfel_post_camera_partials_bytes(W, H) // 8, dtype=torch.float64, device=dev)
+    return partials, torch.empty((3, 3), device=dev), torch.empty((12,), device=dev)
 
 
 class _SurfaceOutputs(torch.autograd.Function):
@@ -72,7 +81,14 @@ class _SurfaceOutputs(torch.autograd.Function):
             _cabi.check(lib.surfel_post_backward(W, H, ctx.depth_ratio, allmap.data_ptr(), rot.data_ptr(), rays.data_ptr(),
                                                  surf_depth.data_ptr(), p(g_rend_normal), p(g_surf_depth), p(g_surf_normal),
                                                  tmp.data_ptr(), g_allmap.data_ptr(), torch.cuda.current_stream(dev).cuda_stream))
-        return g_allmap, None, None, None
+            g_rot, g_rays = None, None
+            if ctx.needs_input_grad[1] or ctx.needs_input_grad[2]:
+                partials, g_rot, g_rays = _camera_buffers(lib, W, H, dev)
+                _cabi.check(lib.surfel_post_camera_backward(
+                    W, H, ctx.depth_ratio, allmap.data_ptr(), rot.data_ptr(), rays.data_ptr(), surf_depth.data_ptr(),
+                    p(g_rend_normal), p(g_surf_depth), p(g_surf_normal), tmp.data_ptr(), partials.data_ptr(),
+                    g_rot.data_ptr(), g_rays.data_ptr(), torch.cuda.current_stream(dev).cuda_stream))
+        return g_allmap, g_rot, g_rays, None
 
 
 class _SurfaceRegularizers(torch.autograd.Function):
@@ -111,7 +127,14 @@ class _SurfaceRegularizers(torch.autograd.Function):
                                                      rot.data_ptr(), rays.data_ptr(), gscale.data_ptr(),
                                                      None if tmp is None else tmp.data_ptr(), g_allmap.data_ptr(),
                                                      torch.cuda.current_stream(dev).cuda_stream))
-        return g_allmap, None, None, None, None, None
+            g_rot, g_rays = None, None
+            if ctx.needs_input_grad[1] or ctx.needs_input_grad[2]:
+                partials, g_rot, g_rays = _camera_buffers(lib, W, H, dev)
+                _cabi.check(lib.surfel_post_reg_camera_backward(
+                    W, H, depth_ratio, lambda_normal, lambda_dist, allmap.data_ptr(), rot.data_ptr(), rays.data_ptr(),
+                    gscale.data_ptr(), None if tmp is None else tmp.data_ptr(), partials.data_ptr(), g_rot.data_ptr(),
+                    g_rays.data_ptr(), torch.cuda.current_stream(dev).cuda_stream))
+        return g_allmap, g_rot, g_rays, None, None, None
 
 
 def _check_inputs(fn, allmap, viewpoint_camera):
@@ -146,8 +169,10 @@ def surface_regularizers(allmap, viewpoint_camera, depth_ratio, lambda_normal, l
         normal_loss = lambda_normal * normal_error.mean()
         dist_loss = lambda_dist * rend_dist.mean()
 
-    Gradients flow to allmap only; surf_normal's alpha is detached, as in the reference, and where D/alpha is not
-    finite (a hole) its term contributes 0 to the gradient, where the reference's is NaN.  lambda_normal and
+    Gradients flow to allmap and, when they require grad, to the camera's world_view_transform and
+    full_proj_transform (only the normal term depends on the camera); surf_normal's alpha is detached, as in the
+    reference, and where D/alpha is not finite (a hole) its term contributes 0 to allmap's gradient, where the
+    reference's is NaN.  lambda_normal and
     lambda_dist are Python numbers: lambda_normal == 0 skips the normal term (its loss and gradient are exactly
     0), and with both 0 nothing reads allmap.  Inputs are checked as surface_outputs checks them."""
     W, H = _check_inputs("surface_regularizers", allmap, viewpoint_camera)

@@ -240,6 +240,25 @@ int surfel_post_reg_backward(int W, int H, float depth_ratio, double lambda_norm
                              const float* allmap, const float* rot, const float* rays, const float* gscale2,
                              float* tmp6, float* g_allmap, void* stream);
 
+/* Camera gradients of the fused tail (DESIGN.md §7q): g_rot9 = dL/drot (9) and g_rays12 = dL/drays (12), in the
+ * layouts of rot and rays above.  Each call takes the arguments of the backward it follows, on the same stream after
+ * it, and reads the tmp6 that backward wrote; partials is device scratch of surfel_post_camera_partials_bytes(W, H)
+ * bytes (0 for a bad size).  surfel_post_camera_backward follows surfel_post_backward: the rotation term needs
+ * g_rend_normal and the ray term g_surf_normal (either may be NULL; its term is then 0).
+ * surfel_post_reg_camera_backward follows surfel_post_reg_backward: with lambda_normal == 0 both outputs are 0 and
+ * nothing launches (tmp6 and partials may then be NULL).  Sums are reduced in double in a fixed order with no
+ * atomics, so repeat calls give bit-identical outputs on any stream.  Neither call writes anything but partials and
+ * its two outputs. */
+size_t surfel_post_camera_partials_bytes(int W, int H);
+int surfel_post_camera_backward(int W, int H, float depth_ratio, const float* allmap, const float* rot,
+                                const float* rays, const float* surf_depth, const float* g_rend_normal,
+                                const float* g_surf_depth, const float* g_surf_normal, const float* tmp6,
+                                double* partials, float* g_rot9, float* g_rays12, void* stream);
+int surfel_post_reg_camera_backward(int W, int H, float depth_ratio, double lambda_normal, double lambda_dist,
+                                    const float* allmap, const float* rot, const float* rays, const float* gscale2,
+                                    const float* tmp6, double* partials, float* g_rot9, float* g_rays12,
+                                    void* stream);
+
 /* OPT-IN fused photometric loss (SURVEY §8f row f2): (1-l)*L1 + l*(1-SSIM) of
  * /root/reference/train.py:73-74 with /root/reference/utils/loss_utils.py:6-7, :43-73 (11x11 Gaussian
  * window, sigma 1.5, zero padding, per channel).  forward: sums2[0] = sum |img-gt|, sums2[1] = sum of
