@@ -89,6 +89,38 @@ uint32_t* mapped_alias(uint32_t* host) {
     return nullptr;
 }
 
+// the checks and parameters both camera entry points share; `name` prefixes the error messages
+bool camera_params(const char* name, const surfel_settings_t* s, int P, int M, const float* means3D,
+                   const float* scales, const float* rotations, const float* transMat_precomp, const float* shs,
+                   int has_colors_precomp, const int32_t* radii, const void* geom_ws, const float* grad_scratch,
+                   const float* dL_dtransMat, double* partials, bool band_ok, const void* out0, const void* out1,
+                   const void* out2, Frame& f, CamBwdParams& p) {
+    if (!frame_of(s, f)) return false;
+    if (P < 0) { surfel_set_error("P < 0"); return false; }
+    if (!band_ok && (f.row0 != 0 || f.row1 != f.gy)) { surfel_set_error("%s: a tile-row band has no camera gradient", name); return false; }
+    if (!partials || !out0 || !out1 || !out2) { surfel_set_error("%s: NULL output or partials", name); return false; }
+    if (P > 0 && (!means3D || !radii || !geom_ws || !grad_scratch)) { surfel_set_error("%s: NULL required input", name); return false; }
+    if (P > 0 && !transMat_precomp && (!scales || !rotations || !dL_dtransMat)) {
+        surfel_set_error("%s: need scales, rotations and dL_dtransMat, or transMat_precomp", name);
+        return false;
+    }
+    const bool sh = !has_colors_precomp && shs != nullptr;
+    if (sh && (s->sh_degree < 0 || s->sh_degree > 3 || (s->sh_degree + 1) * (s->sh_degree + 1) > M)) {
+        surfel_set_error("%s: sh_degree %d unsupported for M=%d", name, s->sh_degree, M);
+        return false;
+    }
+    GeomLayout L = geom_layout(P);
+    const char* g = (const char*)geom_ws;
+    memset(&p, 0, sizeof(p));
+    p.P = P; p.D = s->sh_degree; p.M = M; p.W = f.W; p.H = f.H; p.scale_modifier = s->scale_modifier;
+    p.means3D = means3D; p.scales = scales; p.rotations = rotations; p.shs = shs;
+    p.transMat_precomp = transMat_precomp; p.has_colors_precomp = has_colors_precomp;
+    p.viewmatrix = s->viewmatrix; p.campos = s->campos;
+    p.radii = radii; p.rec = (const float4*)(g + L.rec); p.clamped = (const uint8_t*)(g + L.clamped);
+    p.grad_rec = grad_scratch; p.dL_dtransMat = dL_dtransMat; p.partials = partials;
+    return true;
+}
+
 }  // namespace
 
 extern "C" {
@@ -315,32 +347,27 @@ int surfel_camera_backward(const surfel_settings_t* s, int P, int M, const float
                            const float* grad_scratch, const float* dL_dtransMat, double* partials,
                            float* dL_dviewmatrix, float* dL_dprojmatrix, float* dL_dcampos, void* stream) {
     Frame f;
-    if (!frame_of(s, f)) return 1;
-    if (P < 0) { surfel_set_error("P < 0"); return 1; }
-    if (f.row0 != 0 || f.row1 != f.gy) { surfel_set_error("surfel_camera_backward: a tile-row band has no camera gradient"); return 1; }
-    if (!partials || !dL_dviewmatrix || !dL_dprojmatrix || !dL_dcampos) { surfel_set_error("surfel_camera_backward: NULL output or partials"); return 1; }
-    if (P > 0 && (!means3D || !radii || !geom_ws || !grad_scratch)) { surfel_set_error("surfel_camera_backward: NULL required input"); return 1; }
-    if (P > 0 && !transMat_precomp && (!scales || !rotations || !dL_dtransMat)) {
-        surfel_set_error("surfel_camera_backward: need scales, rotations and dL_dtransMat, or transMat_precomp");
-        return 1;
-    }
-    const bool sh = !has_colors_precomp && shs != nullptr;
-    if (sh && (s->sh_degree < 0 || s->sh_degree > 3 || (s->sh_degree + 1) * (s->sh_degree + 1) > M)) {
-        surfel_set_error("surfel_camera_backward: sh_degree %d unsupported for M=%d", s->sh_degree, M);
-        return 1;
-    }
-    GeomLayout L = geom_layout(P);
-    const char* g = (const char*)geom_ws;
     CamBwdParams p;
-    memset(&p, 0, sizeof(p));
-    p.P = P; p.D = s->sh_degree; p.M = M; p.W = f.W; p.H = f.H; p.scale_modifier = s->scale_modifier;
-    p.means3D = means3D; p.scales = scales; p.rotations = rotations; p.shs = shs;
-    p.transMat_precomp = transMat_precomp; p.has_colors_precomp = has_colors_precomp;
-    p.viewmatrix = s->viewmatrix; p.campos = s->campos;
-    p.radii = radii; p.rec = (const float4*)(g + L.rec); p.clamped = (const uint8_t*)(g + L.clamped);
-    p.grad_rec = grad_scratch; p.dL_dtransMat = dL_dtransMat; p.partials = partials;
+    if (!camera_params("surfel_camera_backward", s, P, M, means3D, scales, rotations, transMat_precomp, shs,
+                       has_colors_precomp, radii, geom_ws, grad_scratch, dL_dtransMat, partials, false,
+                       dL_dviewmatrix, dL_dprojmatrix, dL_dcampos, f, p))
+        return 1;
     p.dL_dviewmatrix = dL_dviewmatrix; p.dL_dprojmatrix = dL_dprojmatrix; p.dL_dcampos = dL_dcampos;
     return launch_camera_bwd(p, (cudaStream_t)stream);
+}
+
+int surfel_camera_backward_sums(const surfel_settings_t* s, int P, int M, const float* means3D, const float* scales,
+                                const float* rotations, const float* transMat_precomp, const float* shs,
+                                int has_colors_precomp, const int32_t* radii, const void* geom_ws,
+                                const float* grad_scratch, const float* dL_dtransMat, double* partials,
+                                double* dL_dviewmatrix, double* dL_dprojmatrix, double* dL_dcampos, void* stream) {
+    Frame f;
+    CamBwdParams p;
+    if (!camera_params("surfel_camera_backward_sums", s, P, M, means3D, scales, rotations, transMat_precomp, shs,
+                       has_colors_precomp, radii, geom_ws, grad_scratch, dL_dtransMat, partials, true,
+                       dL_dviewmatrix, dL_dprojmatrix, dL_dcampos, f, p))
+        return 1;
+    return launch_camera_bwd_sums(p, dL_dviewmatrix, dL_dprojmatrix, dL_dcampos, (cudaStream_t)stream);
 }
 
 int surfel_sh_grad_expand(int P, int M, int sh_degree, const float* means3D, const float* campos,

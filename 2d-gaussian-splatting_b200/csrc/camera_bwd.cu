@@ -14,6 +14,11 @@
 //   dpr[4r] = W/2 G_0[r],  dpr[4r+1] = H/2 G_1[r],  dpr[4r+3] = (W-1)/2 G_0[r] + (H-1)/2 G_1[r] + G_2[r],  dpr[4r+2] = 0.
 // On the transMat_precomp path T and the normal do not depend on the camera: only C is formed.
 //
+// Tile-row bands (DESIGN §7r): every pixel belongs to one band, so a band's record holds partial sums and the rules
+// above, linear in the record, give the band's share of the whole-frame gradient.  launch_camera_bwd_sums runs the
+// same per-splat kernel and hands out the 35 double sums before the final rounding, so that a multi-GPU caller adds
+// the bands in float64 and rounds once.
+//
 // Determinism: splat i belongs to block i / chunk for a chunk that depends on P alone; each thread adds its splats'
 // float32 terms into double registers, the block reduces them in a fixed tree into one double partial per term, and
 // one block adds the partials in block order and rounds each output once.  No atomics: repeat calls are
@@ -159,8 +164,11 @@ __global__ void __launch_bounds__(kCamThreads) camera_bwd_kernel(CamBwdParams p,
     }
 }
 
-__global__ void camera_finish_kernel(int nblocks, int W, int H, const double* __restrict__ partials,
-                                     float* __restrict__ dvm, float* __restrict__ dpr, float* __restrict__ dcam) {
+// the block partials added in block order; projmatrix through ndc2pix.  Out is float (each output rounded once) or
+// double (the sums before rounding, for a caller that adds several tile-row bands first)
+template <typename Out>
+__device__ __forceinline__ void camera_finish(int nblocks, int W, int H, const double* __restrict__ partials,
+                                              Out* __restrict__ dvm, Out* __restrict__ dpr, Out* __restrict__ dcam) {
     __shared__ double s[kCamTerms];
     const int k = threadIdx.x;
     if (k < kCamTerms) {
@@ -177,16 +185,29 @@ __global__ void camera_finish_kernel(int nblocks, int W, int H, const double* __
         else if (c == 1) v = 0.5 * H * G1;
         else if (c == 2) v = 0.0;
         else v = 0.5 * (W - 1) * G0 + 0.5 * (H - 1) * G1 + G2;
-        dpr[k] = (float)v;
-        dvm[k] = (r < 3 && c < 3) ? (float)s[12 + 3 * r + c] : 0.0f;
+        dpr[k] = (Out)v;
+        dvm[k] = (r < 3 && c < 3) ? (Out)s[12 + 3 * r + c] : (Out)0;
     } else if (k < 19) {
-        dcam[k - 16] = (float)s[21 + k - 16];
+        dcam[k - 16] = (Out)s[21 + k - 16];
     }
+}
+
+__global__ void camera_finish_kernel(int nblocks, int W, int H, const double* __restrict__ partials,
+                                     float* __restrict__ dvm, float* __restrict__ dpr, float* __restrict__ dcam) {
+    camera_finish<float>(nblocks, W, H, partials, dvm, dpr, dcam);
+}
+
+__global__ void camera_sums_finish_kernel(int nblocks, int W, int H, const double* __restrict__ partials,
+                                          double* __restrict__ dvm, double* __restrict__ dpr, double* __restrict__ dcam) {
+    camera_finish<double>(nblocks, W, H, partials, dvm, dpr, dcam);
 }
 
 size_t camera_partials_bytes(int P) { return (size_t)std::max(1, cam_blocks(P)) * kCamTerms * sizeof(double); }
 
-int launch_camera_bwd(const CamBwdParams& p, cudaStream_t stream) {
+namespace {
+
+// the per-splat kernel into p.partials; returns the number of partials (blocks) it wrote
+int launch_camera_partials(const CamBwdParams& p, cudaStream_t stream) {
     const int nb = cam_blocks(p.P);
     if (nb > 0) {
         const int chunk = (p.P + nb - 1) / nb;
@@ -194,9 +215,26 @@ int launch_camera_bwd(const CamBwdParams& p, cudaStream_t stream) {
         camera_bwd_kernel<<<nb, kCamThreads, 0, stream>>>(p, chunk);
         SURFEL_CUDA_OK(cudaGetLastError());
     }
+    return nb;
+}
+
+}  // namespace
+
+int launch_camera_bwd(const CamBwdParams& p, cudaStream_t stream) {
+    const int nb = launch_camera_partials(p, stream);
     {
         LaunchScope scope(kStCameraFinish, stream);
         camera_finish_kernel<<<1, 32, 0, stream>>>(nb, p.W, p.H, p.partials, p.dL_dviewmatrix, p.dL_dprojmatrix, p.dL_dcampos);
+        SURFEL_CUDA_OK(cudaGetLastError());
+    }
+    return 0;
+}
+
+int launch_camera_bwd_sums(const CamBwdParams& p, double* dvm, double* dpr, double* dcam, cudaStream_t stream) {
+    const int nb = launch_camera_partials(p, stream);
+    {
+        LaunchScope scope(kStCameraFinish, stream);
+        camera_sums_finish_kernel<<<1, 32, 0, stream>>>(nb, p.W, p.H, p.partials, dvm, dpr, dcam);
         SURFEL_CUDA_OK(cudaGetLastError());
     }
     return 0;

@@ -75,6 +75,8 @@ int launch_sh_grad_expand(int P, int M, int D, const float* means3D, const float
 
 size_t camera_partials_bytes(int P);
 int launch_camera_bwd(const CamBwdParams& p, cudaStream_t stream);
+// the same step with the 35 sums written as double before rounding (p.dL_d* unused): a tile-row band's share
+int launch_camera_bwd_sums(const CamBwdParams& p, double* dvm, double* dpr, double* dcam, cudaStream_t stream);
 
 // binning
 int launch_duplicate_with_keys(int P, int gx, int gy, int row0, int row1, const float4* tmat,

@@ -308,9 +308,11 @@ class _RasterizeGaussians(torch.autograd.Function):
         return grads + (None,)
 
 
-def _backward(ctx, grad_color, grad_allmap, camera):
+def _backward(ctx, grad_color, grad_allmap, camera, camera_sums=False):
     """The backward of both autograd nodes: the eight splat gradients in the order of the node's splat inputs, and,
-    when `camera` is set, (dL_dviewmatrix (16), dL_dprojmatrix (16), dL_dcampos (3)) from surfel_camera_backward."""
+    when `camera` is set, (dL_dviewmatrix (16), dL_dprojmatrix (16), dL_dcampos (3)) from surfel_camera_backward.
+    camera_sums (tile-row bands, surfel_parallel): the camera gradient is instead the (35,) float64 tensor of
+    surfel_camera_backward_sums, the band's sums before rounding, in the same order."""
     _mark("bwd_enter")
     lib = _cabi.load()
     rs = ctx.raster_settings
@@ -368,12 +370,13 @@ def _backward(ctx, grad_color, grad_allmap, camera):
             _ptr(d_tmat), _ptr(d_sh), _ptr(d_scales), _ptr(d_rot), int(LOWPASS_DEPTH_QUIRK), stream))
         if camera:
             partials = torch.empty((lib.surfel_camera_partials_bytes(P) // 8,), dtype=torch.float64, device=dev)
-            out = torch.empty((35,), dtype=torch.float32, device=dev)
-            _cabi.check(lib.surfel_camera_backward(
+            out = torch.empty((35,), dtype=torch.float64 if camera_sums else torch.float32, device=dev)
+            entry = lib.surfel_camera_backward_sums if camera_sums else lib.surfel_camera_backward
+            _cabi.check(entry(
                 ctypes.byref(cs), P, M, _ptr(means3D), _ptr(scales), _ptr(rotations), _ptr(cov3Ds), _ptr(sh),
                 int(has_colors), radii.data_ptr(), geom.data_ptr(), scratch.data_ptr(), _ptr(d_tmat),
                 partials.data_ptr(), out[0:16].data_ptr(), out[16:32].data_ptr(), out[32:35].data_ptr(), stream))
-            cam = (out[0:16], out[16:32], out[32:35])
+            cam = out if camera_sums else (out[0:16], out[16:32], out[32:35])
     _mark("bwd_launched")
     # (means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp)
     return (d_means3D, d_means2D, d_sh, (d_colors if has_colors else None), d_opacity, d_scales, d_rot, d_cov), cam
@@ -383,7 +386,8 @@ class _RasterizeGaussiansCamera(torch.autograd.Function):
     """The same op with the camera as three more differentiable inputs: viewmatrix (4,4), projmatrix (4,4) and campos
     (3), in the row-vector layout of GaussianRasterizationSettings.  rasterize_gaussians routes here only when one of
     them requires grad; the splat gradients are those of _RasterizeGaussians, the camera gradients come from
-    surfel_camera_backward (DESIGN.md §7p).  The whole frame only: a tile-row band would give per-rank partial sums."""
+    surfel_camera_backward (DESIGN.md §7p).  The whole frame only: a tile-row band gives per-rank partial sums, which
+    surfel_parallel.rasterize_tile_band adds across the ranks (DESIGN.md §7r)."""
 
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
@@ -391,7 +395,8 @@ class _RasterizeGaussiansCamera(torch.autograd.Function):
         rs = raster_settings
         if any(getattr(rs, k, None) is not None for k in ("tile_rows", "out_buffers", "out_replicas")):
             raise RuntimeError("diff_surfel_rasterization: camera gradients are not available with tile_rows, "
-                               "out_buffers or out_replicas (a tile-row band holds only part of the frame)")
+                               "out_buffers or out_replicas (a tile-row band holds only part of the frame); "
+                               "surfel_parallel.rasterize_tile_band sums the bands' camera gradients")
         ctx.cam_meta = tuple((t.shape, t.dtype) for t in (viewmatrix, projmatrix, campos))
         rs = rs._replace(viewmatrix=viewmatrix, projmatrix=projmatrix, campos=campos)
         return _RasterizeGaussians.forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations,

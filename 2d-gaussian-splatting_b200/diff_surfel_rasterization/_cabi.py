@@ -79,6 +79,8 @@ SIGNATURES = {
     "surfel_camera_partials_bytes": (c_size_t, [c_int]),
     "surfel_camera_backward": (c_int, [ctypes.POINTER(SurfelSettings), c_int, c_int] + [c_void_p] * 5 + [c_int]
                                + [c_void_p] * 8 + [c_void_p]),
+    "surfel_camera_backward_sums": (c_int, [ctypes.POINTER(SurfelSettings), c_int, c_int] + [c_void_p] * 5 + [c_int]
+                                    + [c_void_p] * 8 + [c_void_p]),
     "surfel_sh_grad_expand": (c_int, [c_int, c_int, c_int] + [c_void_p] * 4 + [c_void_p]),
     "surfel_mark_visible": (c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "surfel_sort_temp_bytes": (c_size_t, [c_size_t]),

@@ -16,7 +16,9 @@ BASELINE.json's configs 4 and 5 name.
    restricted to the band.  The one exchange step is an all-gather of the band outputs (10 planes), done
    IN PLACE in a frame padded to equal bands; in the backward the per-pixel cotangents are read in place
    (no communication) and the per-splat gradients, which are partial sums over the band's pixels, are
-   summed with one all-reduce of the op's flat gradient bucket.
+   summed with one all-reduce of the op's flat gradient bucket.  When the camera requires grad, each rank's
+   camera step gives its band's share as 35 float64 sums, which one float64 all-reduce adds before a single
+   rounding to float32 (DESIGN §7r).
 
 Collectives go through torch.distributed (NCCL over NVLink on GPUs; gloo in the CPU tests).
 """
@@ -202,16 +204,35 @@ def last_exchange_buffers():
     return _last["frame"], _last["grad_bucket"]
 
 
+def reduce_camera_sums(sums: torch.Tensor, world: int, group=None, grad_reduce: str = "all_reduce") -> torch.Tensor:
+    """The camera gradient of a tile-band frame, (35,) float32 in surfel_camera_backward's order (viewmatrix 16,
+    projmatrix 16, campos 3), from this rank's band sums `sums` ((35,) float64, surfel_camera_backward_sums).  The
+    sums are added over the ranks by one in-place float64 all-reduce and rounded to float32 once, so the result is
+    one rounding of the whole frame's sum, the same on every rank.  grad_reduce="none" rounds this rank's partial
+    instead.  "defer" reduces like "all_reduce": what it defers is the splat bucket, and the camera sums never go
+    into that bucket.  Without a process group, or at world 1, nothing is communicated."""
+    if grad_reduce != "none" and world > 1 and dist.is_initialized():
+        dist.all_reduce(sums, op=dist.ReduceOp.SUM, group=group)
+    return sums.to(torch.float32)
+
+
 class _BandFrame(torch.autograd.Function):
     """One oversized frame rendered cooperatively: this rank's band by the CUDA op, the rest by the in-place
-    all-gather.  Wraps the op's own autograd node (same forward / backward code) and adds the exchange."""
+    all-gather.  Wraps the op's own autograd node (same forward / backward code) and adds the exchange.  With the
+    camera tensors given (viewmatrix, projmatrix, campos: they replace the settings' own), they are differentiable
+    inputs too, as in _RasterizeGaussiansCamera, and their gradients are the bands' sums (reduce_camera_sums)."""
 
     @staticmethod
     def forward(ctx, means3D, means2D, sh, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                settings, rank, world, group, grad_reduce, gather="sync"):
+                settings, rank, world, group, grad_reduce, gather="sync", viewmatrix=None, projmatrix=None,
+                campos=None):
         from diff_surfel_rasterization import _RasterizeGaussians, _mark
         H, W = int(settings.image_height), int(settings.image_width)
         _mark("band_enter")
+        ctx.cam_meta = None
+        if viewmatrix is not None:
+            ctx.cam_meta = tuple((t.shape, t.dtype) for t in (viewmatrix, projmatrix, campos))
+            settings = settings._replace(viewmatrix=viewmatrix, projmatrix=projmatrix, campos=campos)
         band = equal_band(H, rank, world)
         # the SH gradient (48 of the 61 floats per splat) is a rank-1 expansion of 3 numbers: the backward leaves
         # it unexpanded, the 16-float bucket is reduced, and the expansion runs once on the sum
@@ -252,9 +273,11 @@ class _BandFrame(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g_color, g_radii, g_allmap):
-        from diff_surfel_rasterization import _RasterizeGaussians
+        from diff_surfel_rasterization import _backward
         world, group, grad_reduce = ctx.band_meta
-        grads = _RasterizeGaussians.backward(ctx, g_color, None, g_allmap)
+        camera = ctx.cam_meta is not None
+        # the camera step runs right after the band backward, on its record, before any collective
+        grads, sums = _backward(ctx, g_color, g_allmap, camera=camera, camera_sums=True)
         _last["grad_bucket"] = ctx.grad_bucket
         _last["sh_expand"] = ctx.sh_expand
         if grad_reduce == "all_reduce" and world > 1 and dist.is_initialized():
@@ -263,7 +286,11 @@ class _BandFrame(torch.autograd.Function):
             ctx.sh_expand()                  # dL_dsh = basis (x) colour gradient (summed over the ranks after "all_reduce")
         # grad_reduce == "defer": the caller reduces last_exchange_buffers()[1] itself and then calls
         # last_sh_expand()() — until then dL_dsh (shs.grad) is unwritten
-        return grads[:8] + (None, None, None, None, None, None)
+        cam = (None, None, None)
+        if camera:
+            g = reduce_camera_sums(sums, world, group, grad_reduce)
+            cam = tuple(t.reshape(shape).to(dtype) for t, (shape, dtype) in zip((g[0:16], g[16:32], g[32:35]), ctx.cam_meta))
+        return grads + (None, None, None, None, None, None) + cam
 
 
 def rasterize_tile_band(rasterizer_cls, settings, rank: int, world: int, group=None, grad_reduce: str = "all_reduce",
@@ -289,6 +316,13 @@ def rasterize_tile_band(rasterizer_cls, settings, rank: int, world: int, group=N
     "fused_multicast" sends ONE store per value to the group's NVSwitch multicast address instead (measured
     slower at N = 2 — 7.6 ms — the switch handles 32-byte multicast writes poorly; kept for comparison).  The
     returned views belong to a ring of two frames and stay valid until the second-next fused call.
+
+    Camera gradients: when grad mode is on and settings.viewmatrix, projmatrix or campos requires grad (the test of
+    rasterize_gaussians), the frame is also differentiable in the camera, in every gather mode.  Each rank forms its
+    band's share of the rasterizer's camera gradient as float64 sums; "all_reduce" and "defer" add them over the ranks
+    with one float64 all-reduce and round once, "none" rounds this rank's share.  Compose any camera-dependent tail
+    (postprocess.surface_outputs / surface_regularizers) on the gathered frame and do NOT reduce its camera gradient:
+    every rank already holds the whole frame, so that part is whole-frame on every rank (DESIGN §7r).
     `rasterizer_cls` is accepted for symmetry with the single-GPU call and is not used."""
     del rasterizer_cls
     if grad_reduce not in ("all_reduce", "none", "defer"):
@@ -299,9 +333,11 @@ def rasterize_tile_band(rasterizer_cls, settings, rank: int, world: int, group=N
     g = lambda k: inputs.get(k) if inputs.get(k) is not None else empty
     if (inputs.get("shs") is None) == (inputs.get("colors_precomp") is None):
         raise Exception("Please provide excatly one of either SHs or precomputed colors!")
+    from diff_surfel_rasterization import _wants_camera_grad
+    cam = (settings.viewmatrix, settings.projmatrix, settings.campos) if _wants_camera_grad(settings) else ()
     color, radii, allmap = _BandFrame.apply(inputs["means3D"], inputs["means2D"], g("shs"), g("colors_precomp"),
                                             inputs["opacities"], g("scales"), g("rotations"), g("cov3D_precomp"),
-                                            settings, rank, world, group, grad_reduce, gather)
+                                            settings, rank, world, group, grad_reduce, gather, *cam)
     works = _last["works"]
 
     def wait():

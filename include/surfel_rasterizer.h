@@ -191,6 +191,19 @@ int surfel_camera_backward(const surfel_settings_t* s, int P, int M, const float
                            const float* grad_scratch, const float* dL_dtransMat, double* partials,
                            float* dL_dviewmatrix, float* dL_dprojmatrix, float* dL_dcampos, void* stream);
 
+/* The same camera step for one tile-row band of a frame split over several GPUs (DESIGN.md §7r), with the same
+ * arguments, and the band accepted.  Every pixel belongs to one band, so a band's gradient record holds partial sums
+ * and the band's camera gradient is its share of the whole frame's.  The 35 outputs are written as double: the sums
+ * before the final rounding, after the ndc2pix map (vm 16, pr 16, campos 3 in the layout above).  Add the bands'
+ * outputs in double and round once.  On the whole frame, each output cast to float equals surfel_camera_backward's
+ * bit for bit.  Splats the band culled (radii == 0) contribute nothing.  Same scratch, ordering and determinism as
+ * surfel_camera_backward. */
+int surfel_camera_backward_sums(const surfel_settings_t* s, int P, int M, const float* means3D, const float* scales,
+                                const float* rotations, const float* transMat_precomp, const float* shs,
+                                int has_colors_precomp, const int32_t* radii, const void* geom_ws,
+                                const float* grad_scratch, const float* dL_dtransMat, double* partials,
+                                double* dL_dviewmatrix, double* dL_dprojmatrix, double* dL_dcampos, void* stream);
+
 /* dL_dsh (P,M,3) = basis_k(normalize(means3D - campos)) * dL_dcolors[c] for k < (sh_degree+1)^2, zero beyond:
  * the expansion surfel_backward() skips when surfel_settings.sh_grad_deferred = 1.  Rows of splats whose
  * colour gradient is exactly zero are zero. */
