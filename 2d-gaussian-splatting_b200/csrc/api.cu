@@ -89,6 +89,9 @@ uint32_t* mapped_alias(uint32_t* host) {
     return nullptr;
 }
 
+// SH degree D is supported (0..3) and its (D + 1)^2 coefficients fit in a row of M
+bool sh_degree_ok(int D, int M) { return D >= 0 && D <= 3 && (D + 1) * (D + 1) <= M; }
+
 // the checks and parameters both camera entry points share; `name` prefixes the error messages
 bool camera_params(const char* name, const surfel_settings_t* s, int P, int M, const float* means3D,
                    const float* scales, const float* rotations, const float* transMat_precomp, const float* shs,
@@ -105,7 +108,7 @@ bool camera_params(const char* name, const surfel_settings_t* s, int P, int M, c
         return false;
     }
     const bool sh = !has_colors_precomp && shs != nullptr;
-    if (sh && (s->sh_degree < 0 || s->sh_degree > 3 || (s->sh_degree + 1) * (s->sh_degree + 1) > M)) {
+    if (sh && !sh_degree_ok(s->sh_degree, M)) {
         surfel_set_error("%s: sh_degree %d unsupported for M=%d", name, s->sh_degree, M);
         return false;
     }
@@ -183,7 +186,7 @@ int surfel_forward_preprocess(const surfel_settings_t* s, int P, int M, const fl
     if (P > 0 && (!means3D || !opacities || !radii || !geom_ws)) { surfel_set_error("NULL required pointer"); return 1; }
     if (P > 0 && !transMat_precomp && (!scales || !rotations)) { surfel_set_error("need scales+rotations or transMat_precomp"); return 1; }
     if (P > 0 && !colors_precomp && !shs) { surfel_set_error("need shs or colors_precomp"); return 1; }
-    if (!colors_precomp && (s->sh_degree < 0 || s->sh_degree > 3 || (s->sh_degree + 1) * (s->sh_degree + 1) > M)) {
+    if (!colors_precomp && !sh_degree_ok(s->sh_degree, M)) {
         surfel_set_error("sh_degree %d unsupported for M=%d coefficients (max degree 3)", s->sh_degree, M);
         return 1;
     }
@@ -374,7 +377,7 @@ int surfel_sh_grad_expand(int P, int M, int sh_degree, const float* means3D, con
                           const float* dL_dcolors, float* dL_dsh, void* stream) {
     if (P <= 0 || M <= 0) return 0;
     if (!means3D || !campos || !dL_dcolors || !dL_dsh) { surfel_set_error("surfel_sh_grad_expand: NULL argument"); return 1; }
-    if (sh_degree < 0 || sh_degree > 3 || (sh_degree + 1) * (sh_degree + 1) > M) { surfel_set_error("surfel_sh_grad_expand: degree / M mismatch"); return 1; }
+    if (!sh_degree_ok(sh_degree, M)) { surfel_set_error("surfel_sh_grad_expand: degree / M mismatch"); return 1; }
     return launch_sh_grad_expand(P, M, sh_degree, means3D, campos, dL_dcolors, dL_dsh, (cudaStream_t)stream);
 }
 

@@ -28,58 +28,17 @@
 #include "common.cuh"
 #include "kernels.h"
 #include "profile.h"
+#include "splat_math.cuh"
 
 namespace surfel {
 
 namespace {
-
-__constant__ float k_SH_C2[5] = {1.0925484305920792f, -1.0925484305920792f, 0.31539156525252005f,
-                                 -1.0925484305920792f, 0.5462742152960396f};
-__constant__ float k_SH_C3[7] = {-0.5900435899266435f, 2.890611442640554f, -0.4570457994644658f,
-                                 0.3731763325901154f,  -0.4570457994644658f, 1.445305721320277f,
-                                 -0.5900435899266435f};
-constexpr float kSH_C1 = 0.4886025119029199f;
 
 constexpr int kCamTerms = 24;          // 12 G, 9 V, 3 C
 constexpr int kCamThreads = 256;
 constexpr int kCamMaxBlocks = 1024;
 
 int cam_blocks(int P) { return P <= 0 ? 0 : std::min(kCamMaxBlocks, (P + kCamThreads - 1) / kCamThreads); }
-
-// d(colour . dR)/d(direction) for the unnormalised direction (dx, dy, dz): the SH part of dL_dmeans3D
-__device__ __forceinline__ void sh_direction_grad(const float* __restrict__ sh, int D, const float dR[3], float dx,
-                                                  float dy, float dz, float g[3]) {
-    const float invl = rsqrtf(dx * dx + dy * dy + dz * dz);
-    const float x = dx * invl, y = dy * invl, z = dz * invl;
-    auto dot = [&](int i) { return dR[0] * __ldg(sh + 3 * i) + dR[1] * __ldg(sh + 3 * i + 1) + dR[2] * __ldg(sh + 3 * i + 2); };
-    float gx = 0.0f, gy = 0.0f, gz = 0.0f;
-    if (D > 0) {
-        const float d1 = dot(1), d2 = dot(2), d3 = dot(3);
-        gx += -kSH_C1 * d3; gy += -kSH_C1 * d1; gz += kSH_C1 * d2;
-        if (D > 1) {
-            const float xx = x * x, yy = y * y, zz = z * z, xy = x * y, yz = y * z, xz = x * z;
-            const float d4 = dot(4), d5 = dot(5), d6 = dot(6), d7 = dot(7), d8 = dot(8);
-            gx += k_SH_C2[0] * y * d4 - k_SH_C2[2] * 2.0f * x * d6 + k_SH_C2[3] * z * d7 + k_SH_C2[4] * 2.0f * x * d8;
-            gy += k_SH_C2[0] * x * d4 + k_SH_C2[1] * z * d5 - k_SH_C2[2] * 2.0f * y * d6 - k_SH_C2[4] * 2.0f * y * d8;
-            gz += k_SH_C2[1] * y * d5 + k_SH_C2[2] * 4.0f * z * d6 + k_SH_C2[3] * x * d7;
-            if (D > 2) {
-                const float d9 = dot(9), d10 = dot(10), d11 = dot(11), d12 = dot(12), d13 = dot(13), d14 = dot(14), d15 = dot(15);
-                gx += k_SH_C3[0] * d9 * 6.0f * xy + k_SH_C3[1] * d10 * yz - k_SH_C3[2] * d11 * 2.0f * xy -
-                      k_SH_C3[3] * d12 * 6.0f * xz + k_SH_C3[4] * d13 * (4.0f * zz - 3.0f * xx - yy) +
-                      k_SH_C3[5] * d14 * 2.0f * xz + k_SH_C3[6] * d15 * 3.0f * (xx - yy);
-                gy += k_SH_C3[0] * d9 * 3.0f * (xx - yy) + k_SH_C3[1] * d10 * xz +
-                      k_SH_C3[2] * d11 * (4.0f * zz - xx - 3.0f * yy) - k_SH_C3[3] * d12 * 6.0f * yz -
-                      k_SH_C3[4] * d13 * 2.0f * xy - k_SH_C3[5] * d14 * 2.0f * yz - k_SH_C3[6] * d15 * 6.0f * xy;
-                gz += k_SH_C3[1] * d10 * xy + k_SH_C3[2] * d11 * 8.0f * yz +
-                      k_SH_C3[3] * d12 * 3.0f * (2.0f * zz - xx - yy) + k_SH_C3[4] * d13 * 8.0f * xz +
-                      k_SH_C3[5] * d14 * (xx - yy);
-            }
-        }
-    }
-    // through the normalisation: (I - u u^T) / |d| applied to (gx, gy, gz)
-    const float ug = x * gx + y * gy + z * gz;
-    g[0] = (gx - x * ug) * invl; g[1] = (gy - y * ug) * invl; g[2] = (gz - z * ug) * invl;
-}
 
 }  // namespace
 
@@ -99,14 +58,16 @@ __global__ void __launch_bounds__(kCamThreads) camera_bwd_kernel(CamBwdParams p,
         const float4 rg = reinterpret_cast<const float4*>(p.grad_rec + (size_t)idx * kGradFloats)[4];   // gn, gc.x
         const float2 rg2 = reinterpret_cast<const float2*>(p.grad_rec + (size_t)idx * kGradFloats)[10];  // gc.yz
         if (geom) {
+            // rsqrtf rounds once; preprocess's 1/sqrtf rounds twice, and where |q|^2 rounds to 1 - 2^-24 that alone moves
+            // a diagonal entry of R near 0.15 by 1.3e-6 of its value, beyond the bound of DESIGN §7p's exact test
             const float4 q = reinterpret_cast<const float4*>(p.rotations)[idx];
+            const QuatRotation qr = quat_rotation(q, rsqrtf(q.x * q.x + q.y * q.y + q.z * q.z + q.w * q.w));
+            const float (&R)[3][3] = qr.R;
             const float2 sc = reinterpret_cast<const float2*>(p.scales)[idx];
-            const float inv = rsqrtf(q.x * q.x + q.y * q.y + q.z * q.z + q.w * q.w);
-            const float w = q.x * inv, x = q.y * inv, y = q.z * inv, z = q.w * inv;
             const float su = p.scale_modifier * sc.x, sv = p.scale_modifier * sc.y;
-            const float L0[3] = {(1.0f - 2.0f * (y * y + z * z)) * su, 2.0f * (x * y + w * z) * su, 2.0f * (x * z - w * y) * su};
-            const float L1[3] = {2.0f * (x * y - w * z) * sv, (1.0f - 2.0f * (x * x + z * z)) * sv, 2.0f * (y * z + w * x) * sv};
-            const float L2[3] = {2.0f * (x * z + w * y), 2.0f * (y * z - w * x), 1.0f - 2.0f * (x * x + y * y)};
+            const float L0[3] = {R[0][0] * su, R[1][0] * su, R[2][0] * su};
+            const float L1[3] = {R[0][1] * sv, R[1][1] * sv, R[2][1] * sv};
+            const float L2[3] = {R[0][2], R[1][2], R[2][2]};
             const float pp[3] = {px, py, pz};
             const float* gT = p.dL_dtransMat + 9 * (size_t)idx;
 #pragma unroll
@@ -135,10 +96,14 @@ __global__ void __launch_bounds__(kCamThreads) camera_bwd_kernel(CamBwdParams p,
             const uint8_t cb = p.clamped[idx];
             const float dR[3] = {(cb & 1) ? 0.0f : rg.w, (cb & 2) ? 0.0f : rg2.x, (cb & 4) ? 0.0f : rg2.y};
             if (p.D > 0 && (dR[0] != 0.0f || dR[1] != 0.0f || dR[2] != 0.0f)) {
-                float g[3];
-                sh_direction_grad(p.shs + (size_t)idx * 3 * p.M, p.D, dR, px - p.campos[0], py - p.campos[1],
-                                  pz - p.campos[2], g);
-                t[21] = -g[0]; t[22] = -g[1]; t[23] = -g[2];
+                // the direction is means3D - campos: minus preprocess backward's SH term of dL_dmeans3D
+                const float* sh = p.shs + (size_t)idx * 3 * p.M;
+                const float dox = px - p.campos[0], doy = py - p.campos[1], doz = pz - p.campos[2];
+                const float invl = 1.0f / sqrtf(dox * dox + doy * doy + doz * doz);
+                const float3 dd = sh_backward(p.D, dox * invl, doy * invl, doz * invl, dR,
+                                              [&](int i, int c) { return __ldg(sh + 3 * i + c); }, [](int, float) {});
+                const float3 g = sh_direction_to_mean(dox, doy, doz, invl, dd);
+                t[21] = -g.x; t[22] = -g.y; t[23] = -g.z;
             }
         }
 #pragma unroll

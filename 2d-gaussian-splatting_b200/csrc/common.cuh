@@ -135,6 +135,15 @@ __device__ __forceinline__ float4 ld_nc_f4(const float4* p) {
     return r;
 }
 
+// 16-byte global -> shared copy that bypasses registers and L1 (LDGSTS), to a shared-window address
+// (__cvta_generic_to_shared), and the wait for all of this thread's copies.
+__device__ __forceinline__ void cp_async16(uint32_t smem_addr, const void* gsrc) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_addr), "l"(gsrc) : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all() {
+    asm volatile("cp.async.commit_group;\ncp.async.wait_group 0;" ::: "memory");
+}
+
 }  // namespace surfel
 
 // Error plumbing shared by the C-ABI translation units.

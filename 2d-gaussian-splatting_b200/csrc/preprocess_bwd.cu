@@ -14,23 +14,9 @@
 #include "common.cuh"
 #include "kernels.h"
 #include "profile.h"
+#include "splat_math.cuh"
 
 namespace surfel {
-
-__constant__ float b_SH_C2[5] = {1.0925484305920792f, -1.0925484305920792f, 0.31539156525252005f,
-                                 -1.0925484305920792f, 0.5462742152960396f};
-__constant__ float b_SH_C3[7] = {-0.5900435899266435f, 2.890611442640554f, -0.4570457994644658f,
-                                 0.3731763325901154f,  -0.4570457994644658f, 1.445305721320277f,
-                                 -0.5900435899266435f};
-constexpr float SH_C0 = 0.28209479177387814f;
-constexpr float SH_C1 = 0.4886025119029199f;
-
-__device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(gsrc) : "memory");
-}
-__device__ __forceinline__ void cp_async_wait_all() {
-    asm volatile("cp.async.commit_group;\ncp.async.wait_group 0;" ::: "memory");
-}
 
 constexpr int kRowQuads = 13;   // 12 data quads + 1 pad: conflict-free 128-bit row access
 
@@ -67,7 +53,7 @@ __global__ void __launch_bounds__(128, 6) preprocess_bwd_kernel(PreBwdParams p) 
         for (int it = 0; it < 12; it++) {
             const int f = it * 32 + lane;
             const int row = f / 12, q = f - row * 12;
-            if ((vis_mask >> row) & 1u) cp_async16(dst + row * kRowQuads + q, src + f);
+            if ((vis_mask >> row) & 1u) cp_async16(__cvta_generic_to_shared(dst + row * kRowQuads + q), src + f);
         }
     }
     float4 rot_in = make_float4(1.0f, 0.0f, 0.0f, 0.0f);
@@ -145,14 +131,10 @@ __global__ void __launch_bounds__(128, 6) preprocess_bwd_kernel(PreBwdParams p) 
             const float* pr = p.projmatrix;
             const float hw = (float)p.W / 2.0f, hh = (float)p.H / 2.0f;
             const float cw = (float)(p.W - 1) / 2.0f, ch = (float)(p.H - 1) / 2.0f;
-            const float4 q = rot_in;
             const float2 sc = scale_in;
-            const float inv = 1.0f / sqrtf(q.x * q.x + q.y * q.y + q.z * q.z + q.w * q.w);
-            const float w = q.x * inv, x = q.y * inv, y = q.z * inv, z = q.w * inv;
-            float R[3][3];
-            R[0][0] = 1.0f - 2.0f * (y * y + z * z); R[0][1] = 2.0f * (x * y - w * z); R[0][2] = 2.0f * (x * z + w * y);
-            R[1][0] = 2.0f * (x * y + w * z); R[1][1] = 1.0f - 2.0f * (x * x + z * z); R[1][2] = 2.0f * (y * z - w * x);
-            R[2][0] = 2.0f * (x * z - w * y); R[2][1] = 2.0f * (y * z + w * x); R[2][2] = 1.0f - 2.0f * (x * x + y * y);
+            const QuatRotation qr = quat_rotation(rot_in);
+            const float w = qr.w, x = qr.x, y = qr.y, z = qr.z;
+            const float (&R)[3][3] = qr.R;
             // dRows[i][k] = sum_j gT[3j+i] * Pm[k][j]
             float dRows[3][3];
 #pragma unroll
@@ -219,51 +201,14 @@ __global__ void __launch_bounds__(128, 6) preprocess_bwd_kernel(PreBwdParams p) 
             const float sq = dox * dox + doy * doy + doz * doz;
             const float invl = 1.0f / sqrtf(sq);
             const float x = dox * invl, y = doy * invl, z = doz * invl;
-            float ddx = 0, ddy = 0, ddz = 0;
-#define SHV(i, c) (kStaged ? v[3 * (i) + (c)] : shg[3 * (i) + (c)])
-#define GS(i, val) do { const float _v = (val); if (kStaged) { v[3 * (i)] = _v * dR[0]; v[3 * (i) + 1] = _v * dR[1]; v[3 * (i) + 2] = _v * dR[2]; } \
-                        else if (emit_sh) { gsh[3 * (i)] = _v * dR[0]; gsh[3 * (i) + 1] = _v * dR[1]; gsh[3 * (i) + 2] = _v * dR[2]; } } while (0)
-#define DOT(i) (dR[0] * SHV(i, 0) + dR[1] * SHV(i, 1) + dR[2] * SHV(i, 2))
-            // every DOT(i) is taken before GS(i) overwrites coefficient i (in-place row)
-            GS(0, SH_C0);
-            if (p.D > 0) {
-                const float d1 = DOT(1), d2 = DOT(2), d3 = DOT(3);
-                GS(1, -SH_C1 * y); GS(2, SH_C1 * z); GS(3, -SH_C1 * x);
-                ddx += -SH_C1 * d3; ddy += -SH_C1 * d1; ddz += SH_C1 * d2;
-                if (p.D > 1) {
-                    const float xx = x * x, yy = y * y, zz = z * z, xy = x * y, yz = y * z, xz = x * z;
-                    const float d4 = DOT(4), d5 = DOT(5), d6 = DOT(6), d7 = DOT(7), d8 = DOT(8);
-                    GS(4, b_SH_C2[0] * xy); GS(5, b_SH_C2[1] * yz); GS(6, b_SH_C2[2] * (2.0f * zz - xx - yy));
-                    GS(7, b_SH_C2[3] * xz); GS(8, b_SH_C2[4] * (xx - yy));
-                    ddx += b_SH_C2[0] * y * d4 + b_SH_C2[2] * 2.0f * -x * d6 + b_SH_C2[3] * z * d7 + b_SH_C2[4] * 2.0f * x * d8;
-                    ddy += b_SH_C2[0] * x * d4 + b_SH_C2[1] * z * d5 + b_SH_C2[2] * 2.0f * -y * d6 + b_SH_C2[4] * 2.0f * -y * d8;
-                    ddz += b_SH_C2[1] * y * d5 + b_SH_C2[2] * 4.0f * z * d6 + b_SH_C2[3] * x * d7;
-                    if (p.D > 2) {
-                        const float d9 = DOT(9), d10 = DOT(10), d11 = DOT(11), d12 = DOT(12), d13 = DOT(13), d14 = DOT(14), d15 = DOT(15);
-                        GS(9, b_SH_C3[0] * y * (3.0f * xx - yy)); GS(10, b_SH_C3[1] * xy * z);
-                        GS(11, b_SH_C3[2] * y * (4.0f * zz - xx - yy));
-                        GS(12, b_SH_C3[3] * z * (2.0f * zz - 3.0f * xx - 3.0f * yy));
-                        GS(13, b_SH_C3[4] * x * (4.0f * zz - xx - yy)); GS(14, b_SH_C3[5] * z * (xx - yy));
-                        GS(15, b_SH_C3[6] * x * (xx - 3.0f * yy));
-                        ddx += b_SH_C3[0] * d9 * 6.0f * xy + b_SH_C3[1] * d10 * yz + b_SH_C3[2] * d11 * -2.0f * xy +
-                               b_SH_C3[3] * d12 * -6.0f * xz + b_SH_C3[4] * d13 * (-3.0f * xx + 4.0f * zz - yy) +
-                               b_SH_C3[5] * d14 * 2.0f * xz + b_SH_C3[6] * d15 * 3.0f * (xx - yy);
-                        ddy += b_SH_C3[0] * d9 * 3.0f * (xx - yy) + b_SH_C3[1] * d10 * xz +
-                               b_SH_C3[2] * d11 * (-3.0f * yy + 4.0f * zz - xx) + b_SH_C3[3] * d12 * -6.0f * yz +
-                               b_SH_C3[4] * d13 * -2.0f * xy + b_SH_C3[5] * d14 * -2.0f * yz + b_SH_C3[6] * d15 * -6.0f * xy;
-                        ddz += b_SH_C3[1] * d10 * xy + b_SH_C3[2] * d11 * 8.0f * yz +
-                               b_SH_C3[3] * d12 * 3.0f * (2.0f * zz - xx - yy) + b_SH_C3[4] * d13 * 8.0f * xz +
-                               b_SH_C3[5] * d14 * (xx - yy);
-                    }
-                }
-            }
-#undef GS
-#undef DOT
-#undef SHV
-            const float inv3 = invl * invl * invl;
-            g3[0] += ((doy * doy + doz * doz) * ddx - doy * dox * ddy - doz * dox * ddz) * inv3;
-            g3[1] += (-dox * doy * ddx + (dox * dox + doz * doz) * ddy - doz * doy * ddz) * inv3;
-            g3[2] += (-dox * doz * ddx - doy * doz * ddy + (dox * dox + doy * doy) * ddz) * inv3;
+            // the staged row is overwritten in place: sh_backward reads a band's coefficients before handing out its basis
+            auto shv = [&](int i, int c) { return kStaged ? v[3 * i + c] : shg[3 * i + c]; };
+            auto gs = [&](int i, float b) {
+                if (kStaged) { v[3 * i] = b * dR[0]; v[3 * i + 1] = b * dR[1]; v[3 * i + 2] = b * dR[2]; }
+                else if (emit_sh) { gsh[3 * i] = b * dR[0]; gsh[3 * i + 1] = b * dR[1]; gsh[3 * i + 2] = b * dR[2]; }
+            };
+            const float3 gm = sh_direction_to_mean(dox, doy, doz, invl, sh_backward(p.D, x, y, z, dR, shv, gs));
+            g3[0] += gm.x; g3[1] += gm.y; g3[2] += gm.z;
         }
         if (!emit_sh) {
             // deferred: the caller expands basis (x) colour gradient itself (surfel_sh_grad_expand), typically
@@ -313,7 +258,7 @@ __global__ void __launch_bounds__(128, 6) preprocess_bwd_kernel(PreBwdParams p) 
 }
 
 // One warp per 32 splats: every lane evaluates the real SH basis of its own splat's view direction into shared
-// memory (the same expressions as the GS(...) lines above), then the warp writes the 32 rows of 3M floats with
+// memory (sh_basis: the basis preprocess backward multiplies), then the warp writes the 32 rows of 3M floats with
 // coalesced stores, each value = basis[k] * dL_dcolor[c].  Splats whose colour gradient is exactly zero (culled
 // everywhere) get zero rows without touching their direction.
 __global__ void __launch_bounds__(128) sh_grad_expand_kernel(int P, int M, int D, const float* __restrict__ means3D,
@@ -333,23 +278,7 @@ __global__ void __launch_bounds__(128) sh_grad_expand_kernel(int P, int M, int D
         const float dox = means3D[3 * (size_t)idx] - campos[0], doy = means3D[3 * (size_t)idx + 1] - campos[1],
                     doz = means3D[3 * (size_t)idx + 2] - campos[2];
         const float invl = 1.0f / sqrtf(dox * dox + doy * doy + doz * doz);
-        const float x = dox * invl, y = doy * invl, z = doz * invl;
-        b[0] = SH_C0;
-        if (D > 0) {
-            b[1] = -SH_C1 * y; b[2] = SH_C1 * z; b[3] = -SH_C1 * x;
-            if (D > 1) {
-                const float xx = x * x, yy = y * y, zz = z * z, xy = x * y, yz = y * z, xz = x * z;
-                b[4] = b_SH_C2[0] * xy; b[5] = b_SH_C2[1] * yz; b[6] = b_SH_C2[2] * (2.0f * zz - xx - yy);
-                b[7] = b_SH_C2[3] * xz; b[8] = b_SH_C2[4] * (xx - yy);
-                if (D > 2) {
-                    b[9] = b_SH_C3[0] * y * (3.0f * xx - yy); b[10] = b_SH_C3[1] * xy * z;
-                    b[11] = b_SH_C3[2] * y * (4.0f * zz - xx - yy);
-                    b[12] = b_SH_C3[3] * z * (2.0f * zz - 3.0f * xx - 3.0f * yy);
-                    b[13] = b_SH_C3[4] * x * (4.0f * zz - xx - yy); b[14] = b_SH_C3[5] * z * (xx - yy);
-                    b[15] = b_SH_C3[6] * x * (xx - 3.0f * yy);
-                }
-            }
-        }
+        sh_basis(D, dox * invl, doy * invl, doz * invl, [&](int i, float v) { b[i] = v; });
     }
 #pragma unroll
     for (int k = 0; k < 16; k++) s_b[warp][lane][k] = b[k];

@@ -21,47 +21,16 @@
 #include "kernels.h"
 #include "profile.h"
 #include "scan.cuh"
+#include "splat_math.cuh"
 
 namespace surfel {
 
-__constant__ float c_SH_C2[5] = {1.0925484305920792f, -1.0925484305920792f, 0.31539156525252005f,
-                                 -1.0925484305920792f, 0.5462742152960396f};
-__constant__ float c_SH_C3[7] = {-0.5900435899266435f, 2.890611442640554f, -0.4570457994644658f,
-                                 0.3731763325901154f,  -0.4570457994644658f, 1.445305721320277f,
-                                 -0.5900435899266435f};
-constexpr float SH_C0 = 0.28209479177387814f;
-constexpr float SH_C1 = 0.4886025119029199f;
-
+// colour channel c of the SH row sh (3 floats per coefficient) in the unit direction (x, y, z): the basis values
+// times the coefficients, added in basis order
 __device__ __forceinline__ float sh_eval_channel(const float* sh, int c, int D, float x, float y, float z) {
-#define S(i) sh[3 * (i) + c]
-    float r = SH_C0 * S(0);
-    if (D > 0) {
-        r = r - SH_C1 * y * S(1) + SH_C1 * z * S(2) - SH_C1 * x * S(3);
-        if (D > 1) {
-            float xx = x * x, yy = y * y, zz = z * z, xy = x * y, yz = y * z, xz = x * z;
-            r = r + c_SH_C2[0] * xy * S(4) + c_SH_C2[1] * yz * S(5) +
-                c_SH_C2[2] * (2.0f * zz - xx - yy) * S(6) + c_SH_C2[3] * xz * S(7) +
-                c_SH_C2[4] * (xx - yy) * S(8);
-            if (D > 2) {
-                r = r + c_SH_C3[0] * y * (3.0f * xx - yy) * S(9) + c_SH_C3[1] * xy * z * S(10) +
-                    c_SH_C3[2] * y * (4.0f * zz - xx - yy) * S(11) +
-                    c_SH_C3[3] * z * (2.0f * zz - 3.0f * xx - 3.0f * yy) * S(12) +
-                    c_SH_C3[4] * x * (4.0f * zz - xx - yy) * S(13) + c_SH_C3[5] * z * (xx - yy) * S(14) +
-                    c_SH_C3[6] * x * (xx - 3.0f * yy) * S(15);
-            }
-        }
-    }
-#undef S
+    float r;
+    sh_basis(D, x, y, z, [&](int i, float b) { r = i == 0 ? b * sh[c] : r + b * sh[3 * i + c]; });
     return r;
-}
-
-// 16-byte global -> shared copy that bypasses registers and L1 (LDGSTS): the SH rows are fetched while
-// the geometry of the same splats is being computed.
-__device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(gsrc) : "memory");
-}
-__device__ __forceinline__ void cp_async_wait_all() {
-    asm volatile("cp.async.commit_group;\ncp.async.wait_group 0;" ::: "memory");
 }
 
 constexpr int kShRowQuads = 13;                 // 12 data quads + 1 pad: conflict-free LDS.128
@@ -133,7 +102,7 @@ __global__ void __launch_bounds__(kPreBlock, SURFEL_PRE_BLOCKS) preprocess_fwd_k
             for (int it = 0; it < 12; it++) {
                 const int f = it * 32 + lane;              // quad f of the warp's contiguous 6 KB of SH
                 const int row = f / 12, q = f - row * 12;
-                if ((prefetched >> row) & 1u) cp_async16(dst + row * kShRowQuads + q, src + f);
+                if ((prefetched >> row) & 1u) cp_async16(__cvta_generic_to_shared(dst + row * kShRowQuads + q), src + f);
             }
         }
     }
@@ -143,18 +112,13 @@ __global__ void __launch_bounds__(kPreBlock, SURFEL_PRE_BLOCKS) preprocess_fwd_k
             const float hw = (float)p.W / 2.0f, hh = (float)p.H / 2.0f;
             const float cw = (float)(p.W - 1) / 2.0f, ch = (float)(p.H - 1) / 2.0f;
             if (p.transMat_precomp == nullptr) {
-                const float4 q = rot_in;
                 const float2 sc = scale_in;
-                const float n2 = ((q.x * q.x + q.y * q.y) + q.z * q.z) + q.w * q.w;
-                const float inv = 1.0f / sqrtf(n2);
-                const float w = q.x * inv, x = q.y * inv, y = q.z * inv, z = q.w * inv;
-                const float R00 = 1.0f - 2.0f * (y * y + z * z), R01 = 2.0f * (x * y - w * z), R02 = 2.0f * (x * z + w * y);
-                const float R10 = 2.0f * (x * y + w * z), R11 = 1.0f - 2.0f * (x * x + z * z), R12 = 2.0f * (y * z - w * x);
-                const float R20 = 2.0f * (x * z - w * y), R21 = 2.0f * (y * z + w * x), R22 = 1.0f - 2.0f * (x * x + y * y);
+                const QuatRotation qr = quat_rotation(rot_in);
+                const float (&R)[3][3] = qr.R;
                 const float su = p.scale_modifier * sc.x, sv = p.scale_modifier * sc.y;
-                const float L0[3] = {R00 * su, R10 * su, R20 * su};
-                const float L1[3] = {R01 * sv, R11 * sv, R21 * sv};
-                const float L2[3] = {R02, R12, R22};
+                const float L0[3] = {R[0][0] * su, R[1][0] * su, R[2][0] * su};
+                const float L1[3] = {R[0][1] * sv, R[1][1] * sv, R[2][1] * sv};
+                const float L2[3] = {R[0][2], R[1][2], R[2][2]};
 #pragma unroll
                 for (int j = 0; j < 3; j++) {
                     float Pm0, Pm1, Pm2, Pm3;

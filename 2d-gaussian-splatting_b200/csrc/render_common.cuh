@@ -125,15 +125,6 @@ __device__ __forceinline__ uint32_t lds32u(uint32_t addr) {
     return v;
 }
 
-// 16-byte global -> shared copy that bypasses registers (LDGSTS): the staging threads of the render
-// kernels keep only the two culling quads of a record in registers.
-__device__ __forceinline__ void cp_async16(uint32_t smem_addr, const void* gsrc) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_addr), "l"(gsrc) : "memory");
-}
-__device__ __forceinline__ void cp_async_wait_all() {
-    asm volatile("cp.async.commit_group;\ncp.async.wait_group 0;" ::: "memory");
-}
-
 // Warp footprint inside a 16x16 tile: 8 (x) by 4 (y) pixels; warp w sits at (w&1, w>>1).
 __device__ __forceinline__ void warp_pixel(int warp, int lane, int& lx, int& ly) {
     lx = ((warp & 1) << 3) + (lane & 7);
