@@ -110,23 +110,8 @@ __global__ void __launch_bounds__(kCamThreads) camera_bwd_kernel(CamBwdParams p,
         for (int k = 0; k < kCamTerms; k++) acc[k] += (double)t[k];
     }
 
-    // fixed-order block reduction: warp butterfly, then the warps' sums in warp order
-    __shared__ double s_red[kCamThreads / 32][kCamTerms];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-    for (int k = 0; k < kCamTerms; k++) {
-        double v = acc[k];
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-        if (lane == 0) s_red[warp][k] = v;
-    }
-    __syncthreads();
-    if (threadIdx.x < kCamTerms) {
-        double s = 0.0;
-#pragma unroll
-        for (int w = 0; w < kCamThreads / 32; w++) s += s_red[w][threadIdx.x];
-        p.partials[(size_t)blockIdx.x * kCamTerms + threadIdx.x] = s;
-    }
+    block_sum<kCamTerms, kCamThreads>(acc, threadIdx.x,
+                                      [&](int k, double v) { p.partials[(size_t)blockIdx.x * kCamTerms + k] = v; });
 }
 
 // the block partials added in block order; projmatrix through ndc2pix.  Out is float (each output rounded once) or

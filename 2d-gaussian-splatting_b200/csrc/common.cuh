@@ -144,6 +144,30 @@ __device__ __forceinline__ void cp_async_wait_all() {
     asm volatile("cp.async.commit_group;\ncp.async.wait_group 0;" ::: "memory");
 }
 
+// Fixed-order block sum of K double terms, called by every thread of a kThreads block (tid: its linear index): a
+// warp butterfly, then the warps' sums in warp order.  Thread k < K hands term k's sum to store(k, sum), so each
+// caller keeps its own partials layout; the order depends on the block shape alone, so the sums are bit-identical
+// across calls.
+template <int K, int kThreads, class Store>
+__device__ __forceinline__ void block_sum(const double (&acc)[K], int tid, Store store) {
+    __shared__ double s_red[kThreads / 32][K];
+    const int lane = tid & 31, warp = tid >> 5;
+#pragma unroll
+    for (int k = 0; k < K; k++) {
+        double v = acc[k];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+        if (lane == 0) s_red[warp][k] = v;
+    }
+    __syncthreads();
+    if (tid < K) {
+        double s = 0.0;
+#pragma unroll
+        for (int w = 0; w < kThreads / 32; w++) s += s_red[w][tid];
+        store(tid, s);
+    }
+}
+
 }  // namespace surfel
 
 // Error plumbing shared by the C-ABI translation units.

@@ -33,16 +33,32 @@ __device__ __forceinline__ float surf_depth_at(const float* __restrict__ allmap,
     return ex * (1.0f - ratio) + ratio * med;
 }
 
+// rend_normal = n_view . Rw at pixel i, n_view the allmap channels 2-4
+__device__ __forceinline__ void rend_normal_at(const float* __restrict__ allmap, const float* __restrict__ rot, int N,
+                                               int i, float r[3]) {
+    const float nx = allmap[2 * N + i], ny = allmap[3 * N + i], nz = allmap[4 * N + i];
+#pragma unroll
+    for (int c = 0; c < 3; c++) r[c] = nx * rot[c] + ny * rot[3 + c] + nz * rot[6 + c];
+}
+
+// the transpose: allmap channels 2-4 of g_allmap from gw, the cotangent of rend_normal, gw . Rw^T
+__device__ __forceinline__ void store_g_view_normal(const float* __restrict__ rot, const float gw[3], int N, int i,
+                                                    float* __restrict__ g_allmap) {
+#pragma unroll
+    for (int k = 0; k < 3; k++) g_allmap[(2 + k) * N + i] = gw[0] * rot[3 * k] + gw[1] * rot[3 * k + 1] + gw[2] * rot[3 * k + 2];
+}
+
 __global__ void post_fwd_depth_normal_kernel(int W, int H, float ratio, const float* __restrict__ allmap,
                                              const float* __restrict__ rot, float* __restrict__ rend_normal,
                                              float* __restrict__ surf_depth) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     const int N = W * H;
     if (i >= N) return;
-    const float nx = allmap[2 * N + i], ny = allmap[3 * N + i], nz = allmap[4 * N + i];
+    float r[3];
+    rend_normal_at(allmap, rot, N, i, r);
     surf_depth[i] = surf_depth_at(allmap, N, i, ratio);
 #pragma unroll
-    for (int c = 0; c < 3; c++) rend_normal[c * N + i] = nx * rot[c] + ny * rot[3 + c] + nz * rot[6 + c];
+    for (int c = 0; c < 3; c++) rend_normal[c * N + i] = r[c];
 }
 
 struct P3 { float x, y, z; };
@@ -54,8 +70,29 @@ __device__ __forceinline__ P3 point_from(float d, const float* __restrict__ rays
     p.z = d * (fx * rays[2] + fy * rays[5] + rays[8]) + rays[11];
     return p;
 }
-__device__ __forceinline__ P3 point_at(const float* __restrict__ depth, const float* __restrict__ rays, int W, int x, int y) {
-    return point_from(depth[y * W + x], rays, x, y);
+
+// dx = P[y+1,x] - P[y-1,x], dy = P[y,x+1] - P[y,x-1] at an interior pixel, the points back-projected from
+// depth(x, y), the surf_depth of pixel (x, y): the plane surface_outputs' forward saved, or recomputed from allmap
+// (the regularisers)
+template <class Depth>
+__device__ __forceinline__ void stencil(int x, int y, const float* __restrict__ rays, const Depth& depth,
+                                        float dx[3], float dy[3]) {
+    const P3 a = point_from(depth(x, y + 1), rays, x, y + 1), b = point_from(depth(x, y - 1), rays, x, y - 1);
+    const P3 c = point_from(depth(x + 1, y), rays, x + 1, y), d = point_from(depth(x - 1, y), rays, x - 1, y);
+    dx[0] = a.x - b.x; dx[1] = a.y - b.y; dx[2] = a.z - b.z;
+    dy[0] = c.x - d.x; dy[1] = c.y - d.y; dy[2] = c.z - d.z;
+}
+
+// v = dx x dy, its length, and surf_normal = normalize(v) * alpha (F.normalize's eps 1e-12)
+struct SurfNormal { float v[3], len, sn[3]; };
+__device__ __forceinline__ SurfNormal surf_normal_from(const float dx[3], const float dy[3], float al) {
+    SurfNormal n;
+    n.v[0] = dx[1] * dy[2] - dx[2] * dy[1]; n.v[1] = dx[2] * dy[0] - dx[0] * dy[2]; n.v[2] = dx[0] * dy[1] - dx[1] * dy[0];
+    n.len = sqrtf(n.v[0] * n.v[0] + n.v[1] * n.v[1] + n.v[2] * n.v[2]);
+    const float inv = 1.0f / fmaxf(n.len, 1e-12f);
+#pragma unroll
+    for (int k = 0; k < 3; k++) n.sn[k] = n.v[k] * inv * al;
+    return n;
 }
 
 // surf_normal = normalize(cross(P[y+1,x]-P[y-1,x], P[y,x+1]-P[y,x-1])) * alpha ; zero on the border
@@ -65,18 +102,14 @@ __global__ void post_fwd_surf_normal_kernel(int W, int H, const float* __restric
     const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
     if (x >= W || y >= H) return;
     const int N = W * H, i = y * W + x;
-    float n0 = 0, n1 = 0, n2 = 0;
+    float sn[3] = {0, 0, 0};
     if (x > 0 && y > 0 && x < W - 1 && y < H - 1) {
-        const P3 a = point_at(surf_depth, rays, W, x, y + 1), b = point_at(surf_depth, rays, W, x, y - 1);
-        const P3 c = point_at(surf_depth, rays, W, x + 1, y), d = point_at(surf_depth, rays, W, x - 1, y);
-        const float dx0 = a.x - b.x, dx1 = a.y - b.y, dx2 = a.z - b.z;
-        const float dy0 = c.x - d.x, dy1 = c.y - d.y, dy2 = c.z - d.z;
-        const float v0 = dx1 * dy2 - dx2 * dy1, v1 = dx2 * dy0 - dx0 * dy2, v2 = dx0 * dy1 - dx1 * dy0;
-        const float inv = 1.0f / fmaxf(sqrtf(v0 * v0 + v1 * v1 + v2 * v2), 1e-12f);
-        const float al = allmap[N + i];
-        n0 = v0 * inv * al; n1 = v1 * inv * al; n2 = v2 * inv * al;
+        float dx[3], dy[3];
+        stencil(x, y, rays, [=](int u, int v) { return surf_depth[v * W + u]; }, dx, dy);
+        const SurfNormal n = surf_normal_from(dx, dy, allmap[N + i]);
+        sn[0] = n.sn[0]; sn[1] = n.sn[1]; sn[2] = n.sn[2];
     }
-    surf_normal[i] = n0; surf_normal[N + i] = n1; surf_normal[2 * N + i] = n2;
+    surf_normal[i] = sn[0]; surf_normal[N + i] = sn[1]; surf_normal[2 * N + i] = sn[2];
 }
 
 // vjp of normalize(v), v = dx x dy, for the normal's cotangent g (alpha already folded in): o = d(dx), d(dy)
@@ -105,14 +138,12 @@ __global__ void post_bwd_normal_vjp_kernel(int W, int H, const float* __restrict
     const int N = W * H, i = y * W + x;
     float o[6] = {0, 0, 0, 0, 0, 0};
     if (x > 0 && y > 0 && x < W - 1 && y < H - 1) {
-        const P3 a = point_at(surf_depth, rays, W, x, y + 1), b = point_at(surf_depth, rays, W, x, y - 1);
-        const P3 c = point_at(surf_depth, rays, W, x + 1, y), d = point_at(surf_depth, rays, W, x - 1, y);
-        const float dx[3] = {a.x - b.x, a.y - b.y, a.z - b.z}, dy[3] = {c.x - d.x, c.y - d.y, c.z - d.z};
-        const float v[3] = {dx[1] * dy[2] - dx[2] * dy[1], dx[2] * dy[0] - dx[0] * dy[2], dx[0] * dy[1] - dx[1] * dy[0]};
-        const float len = sqrtf(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
+        float dx[3], dy[3];
+        stencil(x, y, rays, [=](int u, int v) { return surf_depth[v * W + u]; }, dx, dy);
         const float al = allmap[N + i];                      // alpha is detached in the reference
+        const SurfNormal n = surf_normal_from(dx, dy, al);
         const float g[3] = {g_surf_normal[i] * al, g_surf_normal[N + i] * al, g_surf_normal[2 * N + i] * al};
-        normal_vjp(dx, dy, v, len, g, o);
+        normal_vjp(dx, dy, n.v, n.len, g, o);
     }
 #pragma unroll
     for (int k = 0; k < 6; k++) tmp[k * N + i] = o[k];
@@ -167,8 +198,7 @@ __global__ void post_bwd_allmap_kernel(int W, int H, float ratio, const float* _
     g_allmap[6 * N + i] = 0.0f;
     float gn[3] = {0, 0, 0};
     if (g_rend_normal) { gn[0] = g_rend_normal[i]; gn[1] = g_rend_normal[N + i]; gn[2] = g_rend_normal[2 * N + i]; }
-#pragma unroll
-    for (int k = 0; k < 3; k++) g_allmap[(2 + k) * N + i] = gn[0] * rot[3 * k] + gn[1] * rot[3 * k + 1] + gn[2] * rot[3 * k + 2];
+    store_g_view_normal(rot, gn, N, i, g_allmap);
 }
 
 // ---- the regularisers of train.py (normal consistency and depth distortion), straight from allmap ----------------
@@ -176,63 +206,33 @@ __global__ void post_bwd_allmap_kernel(int W, int H, float ratio, const float* _
 // Neither rend_normal, surf_depth, surf_normal nor a cotangent plane is written: each kernel recomputes the 3x3
 // stencil it needs from allmap, and the backward's only scratch is the 6-plane point gradient of the §7b tail.
 
-// dx = P[y+1,x] - P[y-1,x], dy = P[y,x+1] - P[y,x-1] at an interior pixel, the points back-projected from allmap
-__device__ __forceinline__ void stencil_from_allmap(int W, int x, int y, float ratio, const float* __restrict__ allmap,
-                                                    const float* __restrict__ rays, int N, float dx[3], float dy[3]) {
-    const int i = y * W + x;
-    const P3 a = point_from(surf_depth_at(allmap, N, i + W, ratio), rays, x, y + 1);
-    const P3 b = point_from(surf_depth_at(allmap, N, i - W, ratio), rays, x, y - 1);
-    const P3 c = point_from(surf_depth_at(allmap, N, i + 1, ratio), rays, x + 1, y);
-    const P3 d = point_from(surf_depth_at(allmap, N, i - 1, ratio), rays, x - 1, y);
-    dx[0] = a.x - b.x; dx[1] = a.y - b.y; dx[2] = a.z - b.z;
-    dy[0] = c.x - d.x; dy[1] = c.y - d.y; dy[2] = c.z - d.z;
-}
-
-__device__ __forceinline__ void rend_normal_at(const float* __restrict__ allmap, const float* __restrict__ rot, int N,
-                                               int i, float r[3]) {
-    const float nx = allmap[2 * N + i], ny = allmap[3 * N + i], nz = allmap[4 * N + i];
-#pragma unroll
-    for (int c = 0; c < 3; c++) r[c] = nx * rot[c] + ny * rot[3 + c] + nz * rot[6 + c];
-}
-
 constexpr int kRegThreads = 256;    // the 32x8 block of the other stencil kernels
 
-// forward: per pixel 1 - rend_normal . surf_normal and rend_dist, summed in double per block (fixed order: warp
-// butterfly, then the 8 warps in turn); partials[2b], partials[2b+1] are block b's two sums
+// forward: per pixel 1 - rend_normal . surf_normal and rend_dist, summed in double per block (block_sum);
+// partials[2b], partials[2b+1] are block b's two sums
 __global__ void __launch_bounds__(kRegThreads)
 post_reg_fwd_kernel(int W, int H, float ratio, int with_normal, int with_dist, const float* __restrict__ allmap,
                     const float* __restrict__ rot, const float* __restrict__ rays, double* __restrict__ partials) {
-    __shared__ double red[2][kRegThreads / 32];
     const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
     const int tid = threadIdx.y * blockDim.x + threadIdx.x;
-    double en = 0.0, ed = 0.0;
+    double acc[2] = {0.0, 0.0};     // normal, dist
     if (x < W && y < H) {
         const int N = W * H, i = y * W + x;
         if (with_normal) {
             float sn[3] = {0, 0, 0}, r[3];
             if (x > 0 && y > 0 && x < W - 1 && y < H - 1) {
                 float dx[3], dy[3];
-                stencil_from_allmap(W, x, y, ratio, allmap, rays, N, dx, dy);
-                const float v0 = dx[1] * dy[2] - dx[2] * dy[1], v1 = dx[2] * dy[0] - dx[0] * dy[2], v2 = dx[0] * dy[1] - dx[1] * dy[0];
-                const float inv = 1.0f / fmaxf(sqrtf(v0 * v0 + v1 * v1 + v2 * v2), 1e-12f);
-                const float al = allmap[N + i];
-                sn[0] = v0 * inv * al; sn[1] = v1 * inv * al; sn[2] = v2 * inv * al;
+                stencil(x, y, rays, [=](int u, int v) { return surf_depth_at(allmap, N, v * W + u, ratio); }, dx, dy);
+                const SurfNormal n = surf_normal_from(dx, dy, allmap[N + i]);
+                sn[0] = n.sn[0]; sn[1] = n.sn[1]; sn[2] = n.sn[2];
             }
             rend_normal_at(allmap, rot, N, i, r);
-            en = (double)(1.0f - (r[0] * sn[0] + r[1] * sn[1] + r[2] * sn[2]));
+            acc[0] = (double)(1.0f - (r[0] * sn[0] + r[1] * sn[1] + r[2] * sn[2]));
         }
-        if (with_dist) ed = (double)allmap[6 * N + i];
+        if (with_dist) acc[1] = (double)allmap[6 * N + i];
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) { en += __shfl_xor_sync(0xffffffffu, en, o); ed += __shfl_xor_sync(0xffffffffu, ed, o); }
-    if ((tid & 31) == 0) { red[0][tid >> 5] = en; red[1][tid >> 5] = ed; }
-    __syncthreads();
-    if (tid == 0) {
-        double a = 0.0, b = 0.0;
-        for (int w = 0; w < kRegThreads / 32; w++) { a += red[0][w]; b += red[1][w]; }
-        const int blk = blockIdx.y * gridDim.x + blockIdx.x;
-        partials[2 * blk] = a; partials[2 * blk + 1] = b;
-    }
+    block_sum<2, kRegThreads>(acc, tid,
+                              [&](int k, double v) { partials[2 * (blockIdx.y * gridDim.x + blockIdx.x) + k] = v; });
 }
 
 // one block: each thread sums a fixed stride of the partials in order, then a fixed tree; the values go out as
@@ -270,20 +270,17 @@ __global__ void post_reg_bwd_normal_kernel(int W, int H, float ratio, const floa
     rend_normal_at(allmap, rot, N, i, r);
     if (x > 0 && y > 0 && x < W - 1 && y < H - 1) {
         float dx[3], dy[3];
-        stencil_from_allmap(W, x, y, ratio, allmap, rays, N, dx, dy);
-        const float v[3] = {dx[1] * dy[2] - dx[2] * dy[1], dx[2] * dy[0] - dx[0] * dy[2], dx[0] * dy[1] - dx[1] * dy[0]};
-        const float len = sqrtf(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
-        const float inv = 1.0f / fmaxf(len, 1e-12f);
+        stencil(x, y, rays, [=](int u, int v) { return surf_depth_at(allmap, N, v * W + u, ratio); }, dx, dy);
         const float al = allmap[N + i];                      // alpha is detached in the reference
-        sn[0] = v[0] * inv * al; sn[1] = v[1] * inv * al; sn[2] = v[2] * inv * al;
+        const SurfNormal n = surf_normal_from(dx, dy, al);
+        sn[0] = n.sn[0]; sn[1] = n.sn[1]; sn[2] = n.sn[2];
         const float g[3] = {-s * r[0] * al, -s * r[1] * al, -s * r[2] * al};
-        normal_vjp(dx, dy, v, len, g, o);
+        normal_vjp(dx, dy, n.v, n.len, g, o);
     }
 #pragma unroll
     for (int k = 0; k < 6; k++) tmp[k * N + i] = o[k];
     const float gn[3] = {-s * sn[0], -s * sn[1], -s * sn[2]};
-#pragma unroll
-    for (int k = 0; k < 3; k++) g_allmap[(2 + k) * N + i] = gn[0] * rot[3 * k] + gn[1] * rot[3 * k + 1] + gn[2] * rot[3 * k + 2];
+    store_g_view_normal(rot, gn, N, i, g_allmap);
 }
 
 // backward 2: channels 0, 1 and 5 through the stencil (tmp; all of 0-5 are 0 without the normal term, tmp NULL) and
@@ -307,14 +304,14 @@ __global__ void post_reg_bwd_allmap_kernel(int W, int H, float ratio, const floa
 //   G_rot[3r+c]  = sum_p n_view_r(p) gw_c(p)           gw: the cotangent of rend_normal (world space)
 //   G_rays[3k+j] = sum_p d(p) q_k(p) dP_j(p)           q = (x, y, 1), d = surf_depth, dP the point gradient
 //   G_rays[9+j]  = sum_p dP_j(p)
-// Each thread forms its pixels' 21 float32 terms and adds them into double registers; the block reduces them in a
-// fixed tree into one double partial per term, and one block adds the partials in a fixed order and rounds each
+// Each thread forms its pixels' 21 float32 terms and adds them into double registers; the block reduces them with
+// block_sum into one double partial per term, and one block adds the partials in a fixed order and rounds each
 // output once.  No atomics: repeat calls are bit-identical, on any stream.
 constexpr int kCamTerms = 21;       // 9 rot, 12 rays
 constexpr int kCamRows = 8;         // rows per thread: a 32x8 block covers 32 x 64 pixels
 
-// kReg: the regularisers' backward (gw = -gscale[0] sn, sn formed from allmap as post_reg_bwd_normal_kernel does,
-// d = surf_depth_at); otherwise surface_outputs' (gw = g_rend_normal, may be NULL; d = the saved surf_depth).
+// kReg: the regularisers' backward (gw = -gscale[0] sn, sn the regularisers' surf_normal, surf_depth recomputed from
+// allmap); otherwise surface_outputs' (gw = g_rend_normal, may be NULL; d = the saved surf_depth).
 // tmp NULL: no point gradient (G_rays = 0).  partials: term-major, partials[k * nblocks + block].
 template <bool kReg>
 __global__ void __launch_bounds__(kRegThreads)
@@ -325,6 +322,9 @@ post_camera_kernel(int W, int H, float ratio, const float* __restrict__ allmap, 
 #pragma unroll
     for (int k = 0; k < kCamTerms; k++) acc[k] = 0.0;
     const int N = W * H;
+    const auto depth = [=](int u, int v) {
+        return kReg ? surf_depth_at(allmap, N, v * W + u, ratio) : surf_depth[v * W + u];
+    };
     const int x = blockIdx.x * blockDim.x + threadIdx.x;
     const bool with_rot = kReg || g_rend_normal != nullptr;
     const float s = kReg ? gscale[0] : 0.0f;
@@ -338,12 +338,9 @@ post_camera_kernel(int W, int H, float ratio, const float* __restrict__ allmap, 
                 if (kReg) {
                     if (x > 0 && y > 0 && x < W - 1 && y < H - 1) {
                         float dx[3], dy[3];
-                        stencil_from_allmap(W, x, y, ratio, allmap, rays, N, dx, dy);
-                        const float v0 = dx[1] * dy[2] - dx[2] * dy[1], v1 = dx[2] * dy[0] - dx[0] * dy[2],
-                                    v2 = dx[0] * dy[1] - dx[1] * dy[0];
-                        const float inv = 1.0f / fmaxf(sqrtf(v0 * v0 + v1 * v1 + v2 * v2), 1e-12f);
-                        const float al = allmap[N + i];
-                        gw[0] = -s * (v0 * inv * al); gw[1] = -s * (v1 * inv * al); gw[2] = -s * (v2 * inv * al);
+                        stencil(x, y, rays, depth, dx, dy);
+                        const SurfNormal n = surf_normal_from(dx, dy, allmap[N + i]);
+                        gw[0] = -s * n.sn[0]; gw[1] = -s * n.sn[1]; gw[2] = -s * n.sn[2];
                     }
                 } else {
                     gw[0] = g_rend_normal[i]; gw[1] = g_rend_normal[N + i]; gw[2] = g_rend_normal[2 * N + i];
@@ -357,7 +354,7 @@ post_camera_kernel(int W, int H, float ratio, const float* __restrict__ allmap, 
             if (tmp) {
                 float dP[3];
                 gather_dP(W, H, x, y, tmp, dP);
-                const float d = kReg ? surf_depth_at(allmap, N, i, ratio) : surf_depth[i];
+                const float d = depth(x, y);
                 const float dq[3] = {d * (float)x, d * (float)y, d};
 #pragma unroll
                 for (int k = 0; k < 3; k++)
@@ -369,24 +366,10 @@ post_camera_kernel(int W, int H, float ratio, const float* __restrict__ allmap, 
         }
     }
 
-    // fixed-order block reduction: warp butterfly, then the warps' sums in warp order
-    __shared__ double s_red[kRegThreads / 32][kCamTerms];
-    const int tid = threadIdx.y * blockDim.x + threadIdx.x, lane = tid & 31, warp = tid >> 5;
-#pragma unroll
-    for (int k = 0; k < kCamTerms; k++) {
-        double v = acc[k];
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-        if (lane == 0) s_red[warp][k] = v;
-    }
-    __syncthreads();
-    if (tid < kCamTerms) {
-        double a = 0.0;
-#pragma unroll
-        for (int w = 0; w < kRegThreads / 32; w++) a += s_red[w][tid];
-        const int nblocks = gridDim.x * gridDim.y;
-        partials[(size_t)tid * nblocks + blockIdx.y * gridDim.x + blockIdx.x] = a;
-    }
+    const int tid = threadIdx.y * blockDim.x + threadIdx.x;
+    block_sum<kCamTerms, kRegThreads>(acc, tid, [&](int k, double v) {
+        partials[(size_t)k * (gridDim.x * gridDim.y) + blockIdx.y * gridDim.x + blockIdx.x] = v;
+    });
 }
 
 // one block, one warp per term: lane l adds the partials l, l + 32, ... in order, then a warp butterfly; each output
@@ -409,9 +392,13 @@ post_camera_finish_kernel(int nblocks, const double* __restrict__ partials, floa
 
 using namespace surfel;
 
-// the kernels index the 7 planes of allmap with int, and the 32x8 grid's y extent is limited to 65535
+// the 32x8 block of the stencil kernels (kRegThreads threads) and its grid over the frame
+static const dim3 kPostBlock(32, 8);
+static dim3 post_grid(int W, int H) { return dim3((W + 31) / 32, (H + 7) / 8); }
+
+// the kernels index the 7 planes of allmap with int, and the grid's y extent is limited to 65535
 static bool post_size_ok(int W, int H) {
-    return W > 0 && H > 0 && 7LL * W * H <= 0x7fffffffLL && (H + 7) / 8 <= 65535;
+    return W > 0 && H > 0 && 7LL * W * H <= 0x7fffffffLL && post_grid(W, H).y <= 65535;
 }
 
 extern "C" {
@@ -428,8 +415,8 @@ int surfel_post_forward(int W, int H, float depth_ratio, const float* allmap, co
     prof_count_launch(); prof_count_launch();
     post_fwd_depth_normal_kernel<<<(N + 255) / 256, 256, 0, st>>>(W, H, depth_ratio, allmap, rot, rend_normal, surf_depth);
     SURFEL_CUDA_OK(cudaGetLastError());
-    dim3 blk(32, 8), grd((W + 31) / 32, (H + 7) / 8);
-    post_fwd_surf_normal_kernel<<<grd, blk, 0, st>>>(W, H, allmap, surf_depth, rays, surf_normal);
+    const dim3 grd = post_grid(W, H);
+    post_fwd_surf_normal_kernel<<<grd, kPostBlock, 0, st>>>(W, H, allmap, surf_depth, rays, surf_normal);
     SURFEL_CUDA_OK(cudaGetLastError());
     return 0;
 }
@@ -443,22 +430,23 @@ int surfel_post_backward(int W, int H, float depth_ratio, const float* allmap, c
         surfel_set_error("surfel_post_backward: NULL required pointer"); return 1;
     }
     cudaStream_t st = (cudaStream_t)stream;
-    dim3 blk(32, 8), grd((W + 31) / 32, (H + 7) / 8);
+    const dim3 grd = post_grid(W, H);
     prof_count_launch(); prof_count_launch();
     if (g_surf_normal) {
-        post_bwd_normal_vjp_kernel<<<grd, blk, 0, st>>>(W, H, allmap, surf_depth, rays, g_surf_normal, tmp6);
+        post_bwd_normal_vjp_kernel<<<grd, kPostBlock, 0, st>>>(W, H, allmap, surf_depth, rays, g_surf_normal, tmp6);
     } else {
         SURFEL_CUDA_OK(cudaMemsetAsync(tmp6, 0, (size_t)6 * W * H * 4, st));
     }
     SURFEL_CUDA_OK(cudaGetLastError());
-    post_bwd_allmap_kernel<<<grd, blk, 0, st>>>(W, H, depth_ratio, allmap, rays, rot, tmp6, g_rend_normal, g_surf_depth, g_allmap);
+    post_bwd_allmap_kernel<<<grd, kPostBlock, 0, st>>>(W, H, depth_ratio, allmap, rays, rot, tmp6, g_rend_normal, g_surf_depth, g_allmap);
     SURFEL_CUDA_OK(cudaGetLastError());
     return 0;
 }
 
 size_t surfel_post_reg_partials_bytes(int W, int H) {
     if (!post_size_ok(W, H)) return 0;
-    return (size_t)2 * sizeof(double) * ((W + 31) / 32) * ((H + 7) / 8);
+    const dim3 g = post_grid(W, H);
+    return (size_t)2 * sizeof(double) * g.x * g.y;
 }
 
 int surfel_post_reg_forward(int W, int H, float depth_ratio, double lambda_normal, double lambda_dist,
@@ -474,9 +462,9 @@ int surfel_post_reg_forward(int W, int H, float depth_ratio, double lambda_norma
         SURFEL_CUDA_OK(cudaMemsetAsync(dist_loss, 0, sizeof(float), st));
         return 0;
     }
-    dim3 blk(32, 8), grd((W + 31) / 32, (H + 7) / 8);
+    const dim3 grd = post_grid(W, H);
     prof_count_launch(); prof_count_launch();
-    post_reg_fwd_kernel<<<grd, blk, 0, st>>>(W, H, depth_ratio, lambda_normal != 0.0, lambda_dist != 0.0, allmap, rot,
+    post_reg_fwd_kernel<<<grd, kPostBlock, 0, st>>>(W, H, depth_ratio, lambda_normal != 0.0, lambda_dist != 0.0, allmap, rot,
                                              rays, partials);
     SURFEL_CUDA_OK(cudaGetLastError());
     post_reg_final_kernel<<<1, kRegThreads, 0, st>>>(grd.x * grd.y, W * H, lambda_normal, lambda_dist, partials,
@@ -498,14 +486,14 @@ int surfel_post_reg_backward(int W, int H, float depth_ratio, double lambda_norm
         SURFEL_CUDA_OK(cudaMemsetAsync(g_allmap, 0, (size_t)7 * W * H * sizeof(float), st));
         return 0;
     }
-    dim3 blk(32, 8), grd((W + 31) / 32, (H + 7) / 8);
+    const dim3 grd = post_grid(W, H);
     if (with_normal) {
         prof_count_launch();
-        post_reg_bwd_normal_kernel<<<grd, blk, 0, st>>>(W, H, depth_ratio, allmap, rot, rays, gscale2, tmp6, g_allmap);
+        post_reg_bwd_normal_kernel<<<grd, kPostBlock, 0, st>>>(W, H, depth_ratio, allmap, rot, rays, gscale2, tmp6, g_allmap);
         SURFEL_CUDA_OK(cudaGetLastError());
     }
     prof_count_launch();
-    post_reg_bwd_allmap_kernel<<<grd, blk, 0, st>>>(W, H, depth_ratio, allmap, rays, with_normal ? tmp6 : nullptr,
+    post_reg_bwd_allmap_kernel<<<grd, kPostBlock, 0, st>>>(W, H, depth_ratio, allmap, rays, with_normal ? tmp6 : nullptr,
                                                     gscale2, g_allmap);
     SURFEL_CUDA_OK(cudaGetLastError());
     return 0;
@@ -523,12 +511,12 @@ size_t surfel_post_camera_partials_bytes(int W, int H) {
 static int launch_post_camera(bool reg, int W, int H, float ratio, const float* allmap, const float* rays,
                               const float* surf_depth, const float* g_rend_normal, const float* gscale,
                               const float* tmp, double* partials, float* g_rot9, float* g_rays12, cudaStream_t st) {
-    const dim3 blk(32, 8), grd = post_camera_grid(W, H);
+    const dim3 grd = post_camera_grid(W, H);
     prof_count_launch(); prof_count_launch();
     if (reg) {
-        post_camera_kernel<true><<<grd, blk, 0, st>>>(W, H, ratio, allmap, rays, nullptr, nullptr, gscale, tmp, partials);
+        post_camera_kernel<true><<<grd, kPostBlock, 0, st>>>(W, H, ratio, allmap, rays, nullptr, nullptr, gscale, tmp, partials);
     } else {
-        post_camera_kernel<false><<<grd, blk, 0, st>>>(W, H, ratio, allmap, rays, surf_depth, g_rend_normal, nullptr,
+        post_camera_kernel<false><<<grd, kPostBlock, 0, st>>>(W, H, ratio, allmap, rays, surf_depth, g_rend_normal, nullptr,
                                                        tmp, partials);
     }
     SURFEL_CUDA_OK(cudaGetLastError());
