@@ -152,20 +152,16 @@ __global__ void __launch_bounds__(kChThreads) ch_emit_kernel(long long F, long l
                                                              const double* __restrict__ verts, double thresh,
                                                              const uint32_t* __restrict__ count, uint32_t* ctrl,
                                                              unsigned long long* status, double* __restrict__ out) {
-    __shared__ uint32_t s_warp[kChThreads / 32], s_bid, s_excl[1], s_off[kChThreads];
-    if (threadIdx.x == 0) s_bid = atomicAdd(ctrl, 1u);
-    __syncthreads();
-    const uint32_t bid = s_bid;
+    __shared__ uint32_t s_off[kChThreads];
+    const uint32_t bid = block_ticket(ctrl);
     const long long f0 = (long long)bid * kChThreads;
     const uint32_t mine = f0 + threadIdx.x < F ? count[f0 + threadIdx.x] : 0u;
-    uint32_t total;
-    const uint32_t excl = block_exclusive_scan<kChThreads>(mine, s_warp, total);
-    block_lookback<1>(status, gridDim.x, bid, &total, s_excl);
-    s_off[threadIdx.x] = s_excl[0] + excl;
+    const GridScan s = grid_exclusive_scan<kChThreads>(mine, bid, status);
+    s_off[threadIdx.x] = s.rank;
     __syncthreads();
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     for (int k = warp; k < kChThreads && f0 + k < F; k += kChThreads / 32) {
-        if (s_off[k] == (k + 1 < kChThreads ? s_off[k + 1] : s_excl[0] + total)) continue;   // no points
+        if (s_off[k] == (k + 1 < kChThreads ? s_off[k + 1] : s.base + s.total)) continue;   // no points
         bool ok;
         const Tri t = load_tri(f0 + k, M, faces, verts, thresh, ok);
         unsigned long long base = (unsigned long long)M + s_off[k];
@@ -562,10 +558,8 @@ __global__ void __launch_bounds__(kChThreads) ch_select_kernel(uint32_t n, const
                                                                unsigned long long* status, double* __restrict__ down,
                                                                double* __restrict__ in, double* __restrict__ in_obs,
                                                                uint32_t* __restrict__ obs_down, long long* info) {
-    __shared__ uint32_t s_warp[3][kChThreads / 32], s_bid, s_excl[3];
-    if (threadIdx.x == 0) s_bid = atomicAdd(ctrl, 1u);
-    __syncthreads();
-    const uint32_t bid = s_bid;
+    __shared__ uint32_t s_warp[3][kChThreads / 32], s_excl[3];
+    const uint32_t bid = block_ticket(ctrl);
     const uint32_t i = bid * kChThreads + threadIdx.x;
     double x[3] = {0.0, 0.0, 0.0};
     bool kept = false, inb = false, ob = false;
@@ -609,10 +603,7 @@ __global__ void __launch_bounds__(kChThreads) ch_plane_kernel(uint32_t n, const 
                                                               double p1, double p2, double p3, uint32_t* ctrl,
                                                               unsigned long long* status, double* __restrict__ above,
                                                               uint32_t* __restrict__ above_idx, long long* info) {
-    __shared__ uint32_t s_warp[kChThreads / 32], s_bid, s_excl[1];
-    if (threadIdx.x == 0) s_bid = atomicAdd(ctrl, 1u);
-    __syncthreads();
-    const uint32_t bid = s_bid;
+    const uint32_t bid = block_ticket(ctrl);
     const uint32_t i = bid * kChThreads + threadIdx.x;
     double x[3] = {0.0, 0.0, 0.0};
     bool up = false;
@@ -623,16 +614,13 @@ __global__ void __launch_bounds__(kChThreads) ch_plane_kernel(uint32_t n, const 
                                    __dmul_rn(p3, 1.0));
         up = h > 0.0;
     }
-    uint32_t total;
-    const uint32_t excl = block_exclusive_scan<kChThreads>(up ? 1u : 0u, s_warp, total);
-    block_lookback<1>(status, gridDim.x, bid, &total, s_excl);
+    const GridScan s = grid_exclusive_scan<kChThreads>(up ? 1u : 0u, bid, status);
     if (up) {
-        const uint32_t r = s_excl[0] + excl;
 #pragma unroll
-        for (int a = 0; a < 3; a++) above[3 * (size_t)r + a] = x[a];
-        above_idx[r] = i;
+        for (int a = 0; a < 3; a++) above[3 * (size_t)s.rank + a] = x[a];
+        above_idx[s.rank] = i;
     }
-    if (bid == gridDim.x - 1 && threadIdx.x == 0) info[0] = (long long)s_excl[0] + total;
+    if (s.last && threadIdx.x == 0) info[0] = (long long)s.base + s.total;
 }
 
 __global__ void __launch_bounds__(kChThreads) ch_fill_blue_kernel(long long n, double* __restrict__ color) {
@@ -700,10 +688,6 @@ __global__ void __launch_bounds__(kChThreads) ch_sum_final_kernel(int nb, const 
 
 // ---------------------------------------------------------------------------------------------- host side
 
-unsigned blocks_of(long long n, int per = kChThreads) {
-    return (unsigned)std::max<long long>(1, (n + per - 1) / per);
-}
-
 // sample workspace: [ctrl 64 B][status][count u32 per triangle]
 struct SampleLayout { size_t ctrl, status, count, total; };
 SampleLayout sample_layout(long long F) {
@@ -711,7 +695,7 @@ SampleLayout sample_layout(long long F) {
     const size_t f = (size_t)std::max<long long>(F, 1);
     size_t o = 0;
     L.ctrl = o;   o = align_up(o + 64, 256);
-    L.status = o; o = align_up(o + (size_t)blocks_of(F) * 8, 256);
+    L.status = o; o = align_up(o + (size_t)grid_blocks(F, kChThreads) * 8, 256);
     L.count = o;  o = align_up(o + f * 4, 256);
     L.total = o;
     return L;
@@ -728,8 +712,8 @@ EvalLayout eval_layout(long long N, long long S) {
     size_t o = 0;
     L.ctrl = o;     o = align_up(o + 256, 256);         // [0..1] tickets, [8..13] box (u64 at byte 64)
     L.rounds = o;   o = align_up(o + kRoundBatch * 4, 256);
-    L.status_n = o; o = align_up(o + (size_t)3 * blocks_of(N) * 8, 256);
-    L.status_s = o; o = align_up(o + (size_t)blocks_of(S) * 8, 256);
+    L.status_n = o; o = align_up(o + (size_t)3 * grid_blocks(N, kChThreads) * 8, 256);
+    L.status_s = o; o = align_up(o + (size_t)grid_blocks(S, kChThreads) * 8, 256);
     L.sort = o;     o = align_up(o + radix_sort_workspace_bytes(t), 256);
     L.state = o;    o = align_up(o + n, 256);
     L.pts_a = o;    o = align_up(o + n * 32, 256);
@@ -737,7 +721,7 @@ EvalLayout eval_layout(long long N, long long S) {
     L.pts_b = o;    o = align_up(o + s * 32, 256);
     L.boxes_b = o;  o = align_up(o + boxes_for(s) * 64, 256);
     L.pts_q = o;    o = align_up(o + t * 32, 256);
-    L.partial = o;  o = align_up(o + (size_t)blocks_of((long long)t, kChThreads * kSumPer) * 16, 256);
+    L.partial = o;  o = align_up(o + (size_t)grid_blocks((long long)t, kChThreads * kSumPer) * 16, 256);
     L.total = o;
     L.t = t;
     return L;
@@ -755,22 +739,23 @@ int sort_points(const EvalBufs& B, uint32_t n, const double* xyz, double4* pts, 
     cudaStream_t st = B.st;
     SURFEL_CUDA_OK(cudaMemsetAsync(B.bb(), 0xff, 24, st));
     SURFEL_CUDA_OK(cudaMemsetAsync(B.bb() + 3, 0, 24, st));
+    const unsigned nb = grid_blocks(n, kChThreads);
     {
         LaunchScope scope(stage, st);
-        ch_bbox_kernel<<<std::min<unsigned>(blocks_of(n), (unsigned)current_device_sm_count() * 8), kChThreads, 0, st>>>(
+        ch_bbox_kernel<<<std::min<unsigned>(nb, (unsigned)current_device_sm_count() * 8), kChThreads, 0, st>>>(
             n, xyz, B.bb());
         SURFEL_CUDA_OK(cudaGetLastError());
     }
     const RadixSortWs sort = radix_sort_ws(B.w + B.L->sort, B.L->t, 63);
     {
         LaunchScope scope(stage, st);
-        ch_morton_kernel<<<blocks_of(n), kChThreads, 0, st>>>(n, xyz, B.bb(), sort.in.keys, sort.in.vals);
+        ch_morton_kernel<<<nb, kChThreads, 0, st>>>(n, xyz, B.bb(), sort.in.keys, sort.in.vals);
         SURFEL_CUDA_OK(cudaGetLastError());
     }
     if (launch_radix_sort_pairs(sort, n, st)) return 1;
     {
         LaunchScope scope(stage, st);
-        ch_gather_kernel<<<blocks_of(n), kChThreads, 0, st>>>(n, xyz, sort.out.vals, pts);
+        ch_gather_kernel<<<nb, kChThreads, 0, st>>>(n, xyz, sort.out.vals, pts);
         SURFEL_CUDA_OK(cudaGetLastError());
     }
     return 0;
@@ -781,7 +766,7 @@ int build_tree(const EvalBufs& B, uint32_t n, const double* xyz, double4* pts, d
     t = tree_of(n, pts, boxes);
     for (int l = 0; l <= t.top; l++) {
         LaunchScope scope(stage, B.st);
-        ch_box_kernel<<<blocks_of((long long)t.cnt[l] * 32), kChThreads, 0, B.st>>>(l, t, (double4*)boxes);
+        ch_box_kernel<<<grid_blocks((long long)t.cnt[l] * 32, kChThreads), kChThreads, 0, B.st>>>(l, t, boxes);
         SURFEL_CUDA_OK(cudaGetLastError());
     }
     return 0;
@@ -793,12 +778,6 @@ bool eval_sizes_ok(const char* who, long long N, long long S) {
         surfel_set_error("%s: %lld points and %lld STL points; at most %lld each are supported", who, N, S, kChMaxPoints);
         return false;
     }
-    return true;
-}
-
-bool workspace_ok(const char* who, const void* ws, size_t bytes, size_t need) {
-    if (!ws) { surfel_set_error("%s: NULL workspace", who); return false; }
-    if (bytes < need) { surfel_set_error("%s: workspace of %zu bytes, %zu needed", who, bytes, need); return false; }
     return true;
 }
 
@@ -836,14 +815,14 @@ int surfel_chamfer_sample_count(long long n_verts, long long n_faces, const doub
     SURFEL_CUDA_OK(cudaMemsetAsync(info, 0, 4 * sizeof(long long), st));
     if (n_verts > 0) {
         LaunchScope scope(kStChamferSample, st);
-        ch_finite_kernel<<<blocks_of(n_verts), kChThreads, 0, st>>>(n_verts, verts, (unsigned long long*)info + 2);
+        ch_finite_kernel<<<grid_blocks(n_verts, kChThreads), kChThreads, 0, st>>>(n_verts, verts,
+                                                                                  (unsigned long long*)info + 2);
         SURFEL_CUDA_OK(cudaGetLastError());
     }
     if (n_faces > 0) {
         LaunchScope scope(kStChamferSample, st);
-        ch_count_kernel<<<blocks_of(n_faces * 32), kChThreads, 0, st>>>(n_faces, n_verts, faces, verts, thresh,
-                                                                         (uint32_t*)(w + L.count),
-                                                                         (unsigned long long*)info);
+        ch_count_kernel<<<grid_blocks(n_faces * 32, kChThreads), kChThreads, 0, st>>>(
+            n_faces, n_verts, faces, verts, thresh, (uint32_t*)(w + L.count), (unsigned long long*)info);
         SURFEL_CUDA_OK(cudaGetLastError());
     }
     return 0;
@@ -866,11 +845,11 @@ int surfel_chamfer_sample_emit(long long n_verts, long long n_faces, const doubl
     cudaStream_t st = (cudaStream_t)stream;
     char* w = (char*)workspace;
     SURFEL_CUDA_OK(cudaMemsetAsync(w + L.ctrl, 0, 64, st));
-    SURFEL_CUDA_OK(cudaMemsetAsync(w + L.status, 0, (size_t)blocks_of(n_faces) * 8, st));
+    const unsigned nb = grid_blocks(n_faces, kChThreads);
+    SURFEL_CUDA_OK(cudaMemsetAsync(w + L.status, 0, (size_t)nb * 8, st));
     LaunchScope scope(kStChamferSample, st);
-    ch_emit_kernel<<<blocks_of(n_faces), kChThreads, 0, st>>>(n_faces, n_verts, faces, verts, thresh,
-                                                               (const uint32_t*)(w + L.count), (uint32_t*)(w + L.ctrl),
-                                                               (unsigned long long*)(w + L.status), out);
+    ch_emit_kernel<<<nb, kChThreads, 0, st>>>(n_faces, n_verts, faces, verts, thresh, (const uint32_t*)(w + L.count),
+                                              (uint32_t*)(w + L.ctrl), (unsigned long long*)(w + L.status), out);
     SURFEL_CUDA_OK(cudaGetLastError());
     return 0;
 }
@@ -902,7 +881,8 @@ int surfel_chamfer_downsample(long long n_points, long long n_stl, const double*
         SURFEL_CUDA_OK(cudaMemsetAsync(undecided, 0, kRoundBatch * 4, st));
         for (int r = 0; r < kRoundBatch; r++) {
             LaunchScope scope(kStChamferDownsample, st);
-            ch_round_kernel<<<blocks_of((long long)t.cnt[0] * 32), kChThreads, 0, st>>>(t, r2, state, undecided, r);
+            ch_round_kernel<<<grid_blocks((long long)t.cnt[0] * 32, kChThreads), kChThreads, 0, st>>>(t, r2, state,
+                                                                                                    undecided, r);
             SURFEL_CUDA_OK(cudaGetLastError());
         }
         uint32_t left[kRoundBatch];
@@ -944,20 +924,21 @@ int surfel_chamfer_select(long long n_points, long long n_stl, const double* pcd
     char* w = (char*)workspace;
     uint32_t* ctrl = (uint32_t*)(w + L.ctrl);
     SURFEL_CUDA_OK(cudaMemsetAsync(ctrl, 0, 8, st));
-    SURFEL_CUDA_OK(cudaMemsetAsync(w + L.status_n, 0, (size_t)3 * blocks_of(n_points) * 8, st));
-    SURFEL_CUDA_OK(cudaMemsetAsync(w + L.status_s, 0, (size_t)blocks_of(n_stl) * 8, st));
+    const unsigned nb_n = grid_blocks(n_points, kChThreads), nb_s = grid_blocks(n_stl, kChThreads);
+    SURFEL_CUDA_OK(cudaMemsetAsync(w + L.status_n, 0, (size_t)3 * nb_n * 8, st));
+    SURFEL_CUDA_OK(cudaMemsetAsync(w + L.status_s, 0, (size_t)nb_s * 8, st));
     {
         LaunchScope scope(kStChamferSelect, st);
-        ch_select_kernel<<<blocks_of(n_points), kChThreads, 0, st>>>(
+        ch_select_kernel<<<nb_n, kChThreads, 0, st>>>(
             (uint32_t)n_points, pcd, (const uint8_t*)(w + L.state), sp, obs_mask, ctrl,
             (unsigned long long*)(w + L.status_n), data_down, data_in, data_in_obs, obs_down, info);
         SURFEL_CUDA_OK(cudaGetLastError());
     }
     {
         LaunchScope scope(kStChamferSelect, st);
-        ch_plane_kernel<<<blocks_of(n_stl), kChThreads, 0, st>>>((uint32_t)n_stl, stl, plane[0], plane[1], plane[2],
-                                                                 plane[3], ctrl + 1, (unsigned long long*)(w + L.status_s),
-                                                                 stl_above, above_idx, info + 3);
+        ch_plane_kernel<<<nb_s, kChThreads, 0, st>>>((uint32_t)n_stl, stl, plane[0], plane[1], plane[2], plane[3],
+                                                     ctrl + 1, (unsigned long long*)(w + L.status_s), stl_above,
+                                                     above_idx, info + 3);
         SURFEL_CUDA_OK(cudaGetLastError());
     }
     return 0;
@@ -990,12 +971,12 @@ int surfel_chamfer_distances(long long n_points, long long n_stl, const double* 
     double2* partial = (double2*)(B.w + L.partial);
     {
         LaunchScope scope(kStChamferNn, st);
-        ch_fill_blue_kernel<<<blocks_of(n_down), kChThreads, 0, st>>>(n_down, data_color);
+        ch_fill_blue_kernel<<<grid_blocks(n_down, kChThreads), kChThreads, 0, st>>>(n_down, data_color);
         SURFEL_CUDA_OK(cudaGetLastError());
     }
     {
         LaunchScope scope(kStChamferNn, st);
-        ch_fill_blue_kernel<<<blocks_of(n_stl), kChThreads, 0, st>>>(n_stl, stl_color);
+        ch_fill_blue_kernel<<<grid_blocks(n_stl, kChThreads), kChThreads, 0, st>>>(n_stl, stl_color);
         SURFEL_CUDA_OK(cudaGetLastError());
     }
     // d2s: data_in_obs against all of the STL
@@ -1005,8 +986,8 @@ int surfel_chamfer_distances(long long n_points, long long n_stl, const double* 
     if (sort_points(B, (uint32_t)n_obs, data_in_obs, q, kStChamferNn)) return 1;
     {
         LaunchScope scope(kStChamferNn, st);
-        ch_nn_kernel<<<blocks_of(n_obs), kChThreads, 0, st>>>((uint32_t)n_obs, q, ts, max_dist, vis, obs_down, dist_d2s,
-                                                              data_color);
+        ch_nn_kernel<<<grid_blocks(n_obs, kChThreads), kChThreads, 0, st>>>((uint32_t)n_obs, q, ts, max_dist, vis,
+                                                                            obs_down, dist_d2s, data_color);
         SURFEL_CUDA_OK(cudaGetLastError());
     }
     // s2d: stl_above against data_in
@@ -1015,14 +996,14 @@ int surfel_chamfer_distances(long long n_points, long long n_stl, const double* 
     if (sort_points(B, (uint32_t)n_above, stl_above, q, kStChamferNn)) return 1;
     {
         LaunchScope scope(kStChamferNn, st);
-        ch_nn_kernel<<<blocks_of(n_above), kChThreads, 0, st>>>((uint32_t)n_above, q, ti, max_dist, vis, above_idx,
-                                                                dist_s2d, stl_color);
+        ch_nn_kernel<<<grid_blocks(n_above, kChThreads), kChThreads, 0, st>>>((uint32_t)n_above, q, ti, max_dist, vis,
+                                                                              above_idx, dist_s2d, stl_color);
         SURFEL_CUDA_OK(cudaGetLastError());
     }
     const long long ns[2] = {n_obs, n_above};
     const double* ds[2] = {dist_d2s, dist_s2d};
     for (int k = 0; k < 2; k++) {
-        const unsigned nb = blocks_of(ns[k], kChThreads * kSumPer);
+        const unsigned nb = grid_blocks(ns[k], kChThreads * kSumPer);
         {
             LaunchScope scope(kStChamferNn, st);
             ch_sum_kernel<<<nb, kChThreads, 0, st>>>((uint32_t)ns[k], ds[k], max_dist, partial);

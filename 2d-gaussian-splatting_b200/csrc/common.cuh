@@ -173,6 +173,13 @@ __device__ __forceinline__ void block_sum(const double (&acc)[K], int tid, Store
 // Error plumbing shared by the C-ABI translation units.
 void surfel_set_error(const char* fmt, ...);
 
+// Whether `ws` is a workspace of at least `need` bytes; if not, sets the error of entry point `who`.
+inline bool workspace_ok(const char* who, const void* ws, size_t bytes, size_t need) {
+    if (!ws) { surfel_set_error("%s: NULL workspace", who); return false; }
+    if (bytes < need) { surfel_set_error("%s: workspace of %zu bytes, %zu needed", who, bytes, need); return false; }
+    return true;
+}
+
 // Per-device one-time initialisation (function attributes and __constant__ tables live per device, and a
 // process may drive several): slot of the current device in a caller-owned `static bool done[kMaxDevices]`,
 // or -1 if it cannot be determined (then the caller initialises again; all such initialisations are idempotent).

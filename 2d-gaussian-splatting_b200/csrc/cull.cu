@@ -40,7 +40,6 @@ constexpr int kCuMaxSide = 1 << 15;
 constexpr long long kCuMaxCount = (1ll << 31) - 1; // ranks and counts travel in 32 bits, ~0u marks "dropped"
 constexpr uint32_t kDropped = 0xffffffffu;
 
-int blocks_of(long long n) { return (int)std::max<long long>(1, (n + kCuThreads - 1) / kCuThreads); }
 __host__ __device__ inline int words_of(int width) { return (width + 31) / 32; }
 
 // ---- dilation ----
@@ -170,11 +169,8 @@ __global__ void __launch_bounds__(kCuThreads) cu_vertices_kernel(long long M, co
                                                                  uint32_t* __restrict__ vnew, uint32_t* ctrl,
                                                                  unsigned long long* status, long long* info) {
     extern __shared__ float s_proj[];
-    __shared__ uint32_t s_warp[kCuThreads / 32], s_bid, s_excl[1];
     for (int i = threadIdx.x; i < 12 * n_views; i += kCuThreads) s_proj[i] = proj[i];
-    if (threadIdx.x == 0) s_bid = atomicAdd(&ctrl[0], 1u);
-    __syncthreads();
-    const uint32_t bid = s_bid;
+    const uint32_t bid = block_ticket(&ctrl[0]);
     const long long v = (long long)bid * kCuThreads + threadIdx.x;
     bool kept = false;
     if (v < M) {
@@ -184,11 +180,9 @@ __global__ void __launch_bounds__(kCuThreads) cu_vertices_kernel(long long M, co
         kept = vertex_kept(x, y, z, n_views, s_proj, cv, dilated);
         keep[v] = kept ? 1 : 0;
     }
-    uint32_t total;
-    const uint32_t excl = block_exclusive_scan<kCuThreads>(kept ? 1u : 0u, s_warp, total);
-    block_lookback<1>(status, gridDim.x, bid, &total, s_excl);
-    if (v < M) vnew[v] = kept ? s_excl[0] + excl : kDropped;
-    if (bid == gridDim.x - 1 && threadIdx.x == 0) info[2] = (long long)s_excl[0] + total;
+    const GridScan s = grid_exclusive_scan<kCuThreads>(kept ? 1u : 0u, bid, status);
+    if (v < M) vnew[v] = kept ? s.rank : kDropped;
+    if (s.last && threadIdx.x == 0) info[2] = (long long)s.base + s.total;
 }
 
 // info: [0] |= 1 on a face index outside [0, M), [3] = the number of kept faces
@@ -197,10 +191,7 @@ __global__ void __launch_bounds__(kCuThreads) cu_faces_kernel(long long F, long 
                                                               const uint32_t* __restrict__ vnew,
                                                               uint32_t* __restrict__ frank, uint32_t* ctrl,
                                                               unsigned long long* status, long long* info) {
-    __shared__ uint32_t s_warp[kCuThreads / 32], s_bid, s_excl[1];
-    if (threadIdx.x == 0) s_bid = atomicAdd(&ctrl[1], 1u);
-    __syncthreads();
-    const uint32_t bid = s_bid;
+    const uint32_t bid = block_ticket(&ctrl[1]);
     const long long f = (long long)bid * kCuThreads + threadIdx.x;
     bool kept = false;
     if (f < F) {
@@ -215,11 +206,9 @@ __global__ void __launch_bounds__(kCuThreads) cu_faces_kernel(long long F, long 
         }
         if (!ok) atomicOr((unsigned long long*)info, 1ull);
     }
-    uint32_t total;
-    const uint32_t excl = block_exclusive_scan<kCuThreads>(kept ? 1u : 0u, s_warp, total);
-    block_lookback<1>(status, gridDim.x, bid, &total, s_excl);
-    if (f < F) frank[f] = kept ? s_excl[0] + excl : kDropped;
-    if (bid == gridDim.x - 1 && threadIdx.x == 0) info[3] = (long long)s_excl[0] + total;
+    const GridScan s = grid_exclusive_scan<kCuThreads>(kept ? 1u : 0u, bid, status);
+    if (f < F) frank[f] = kept ? s.rank : kDropped;
+    if (s.last && threadIdx.x == 0) info[3] = (long long)s.base + s.total;
 }
 
 struct CuWorld { double s, t[3]; };
@@ -259,8 +248,8 @@ CuLayout cu_layout(long long n_views, int height, int width, long long M, long l
     CuLayout L;
     size_t o = 0;
     L.ctrl = o;     o = align_up(o + 64, 256);
-    L.status_m = o; o = align_up(o + (size_t)blocks_of(M) * 8, 256);
-    L.status_f = o; o = align_up(o + (size_t)blocks_of(F) * 8, 256);
+    L.status_m = o; o = align_up(o + (size_t)grid_blocks(M, kCuThreads) * 8, 256);
+    L.status_f = o; o = align_up(o + (size_t)grid_blocks(F, kCuThreads) * 8, 256);
     L.vnew = o;     o = align_up(o + (size_t)std::max<long long>(M, 1) * 4, 256);
     L.frank = o;    o = align_up(o + (size_t)std::max<long long>(F, 1) * 4, 256);
     L.dist = o;     o = align_up(o + (size_t)n_views * height * width, 256);
@@ -279,15 +268,6 @@ bool sizes_ok(const char* who, long long n_views, int height, int width, long lo
     }
     if (M < 0 || F < 0 || M > kCuMaxCount || F > kCuMaxCount) {
         surfel_set_error("%s: %lld vertices, %lld faces; 0 to %lld of each are supported", who, M, F, kCuMaxCount);
-        return false;
-    }
-    return true;
-}
-
-bool workspace_ok(const char* who, const void* ws, size_t bytes, size_t need) {
-    if (!ws) { surfel_set_error("%s: NULL workspace", who); return false; }
-    if (bytes < need) {
-        surfel_set_error("%s: workspace of %zu bytes, %zu needed", who, bytes, need);
         return false;
     }
     return true;
@@ -363,8 +343,9 @@ int surfel_cull_vertices(long long n_verts, const double* verts, long long n_fac
     uint32_t* ctrl = (uint32_t*)(w + L.ctrl);
     SURFEL_CUDA_OK(cudaMemsetAsync(info, 0, 4 * sizeof(long long), st));
     SURFEL_CUDA_OK(cudaMemsetAsync(ctrl, 0, 64, st));
-    SURFEL_CUDA_OK(cudaMemsetAsync(w + L.status_m, 0, (size_t)blocks_of(n_verts) * 8, st));
-    SURFEL_CUDA_OK(cudaMemsetAsync(w + L.status_f, 0, (size_t)blocks_of(n_faces) * 8, st));
+    const unsigned nb_m = grid_blocks(n_verts, kCuThreads), nb_f = grid_blocks(n_faces, kCuThreads);
+    SURFEL_CUDA_OK(cudaMemsetAsync(w + L.status_m, 0, (size_t)nb_m * 8, st));
+    SURFEL_CUDA_OK(cudaMemsetAsync(w + L.status_f, 0, (size_t)nb_f * 8, st));
     CuView cv;
     cv.img_w1 = (float)(image_width - 1);
     cv.img_h1 = (float)(image_height - 1);
@@ -375,16 +356,16 @@ int surfel_cull_vertices(long long n_verts, const double* verts, long long n_fac
     cv.nw = words_of(width);
     {
         LaunchScope scope(kStCullVertices, st);
-        cu_vertices_kernel<<<blocks_of(n_verts), kCuThreads, (size_t)n_views * 12 * sizeof(float), st>>>(
+        cu_vertices_kernel<<<nb_m, kCuThreads, (size_t)n_views * 12 * sizeof(float), st>>>(
             n_verts, verts, n_views, proj, cv, dilated, keep, (uint32_t*)(w + L.vnew), ctrl,
             (unsigned long long*)(w + L.status_m), info);
         SURFEL_CUDA_OK(cudaGetLastError());
     }
     {
         LaunchScope scope(kStCullFaces, st);
-        cu_faces_kernel<<<blocks_of(n_faces), kCuThreads, 0, st>>>(n_faces, n_verts, faces, (uint32_t*)(w + L.vnew),
-                                                                   (uint32_t*)(w + L.frank), ctrl,
-                                                                   (unsigned long long*)(w + L.status_f), info);
+        cu_faces_kernel<<<nb_f, kCuThreads, 0, st>>>(n_faces, n_verts, faces, (uint32_t*)(w + L.vnew),
+                                                     (uint32_t*)(w + L.frank), ctrl,
+                                                     (unsigned long long*)(w + L.status_f), info);
         SURFEL_CUDA_OK(cudaGetLastError());
     }
     return 0;
@@ -425,14 +406,14 @@ int surfel_cull_emit(long long n_verts, const double* verts, long long n_faces, 
     wt.t[2] = world[3];
     if (n_kept_verts > 0) {
         LaunchScope scope(kStCullEmit, st);
-        cu_emit_vertices_kernel<<<blocks_of(n_verts), kCuThreads, 0, st>>>(
+        cu_emit_vertices_kernel<<<grid_blocks(n_verts, kCuThreads), kCuThreads, 0, st>>>(
             n_verts, verts, (const uint32_t*)(w + L.vnew), wt, (const unsigned char*)colors, color_row_bytes,
             out_verts, (unsigned char*)out_colors);
         SURFEL_CUDA_OK(cudaGetLastError());
     }
     if (n_kept_faces > 0) {
         LaunchScope scope(kStCullEmit, st);
-        cu_emit_faces_kernel<<<blocks_of(n_faces), kCuThreads, 0, st>>>(
+        cu_emit_faces_kernel<<<grid_blocks(n_faces, kCuThreads), kCuThreads, 0, st>>>(
             n_faces, faces, (const uint32_t*)(w + L.vnew), (const uint32_t*)(w + L.frank), out_faces);
         SURFEL_CUDA_OK(cudaGetLastError());
     }

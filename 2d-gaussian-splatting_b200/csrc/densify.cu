@@ -42,15 +42,15 @@ constexpr int kDensifyMaxP = (1 << 30) - 1;       // P' <= 2P must fit an int32 
 
 struct DensifyLayout {
     size_t ctrl, status, rec, total;
-    int blocks;
+    unsigned blocks;
 };
 
 static DensifyLayout densify_layout(int P) {
     DensifyLayout L;
-    L.blocks = P > 0 ? (P + kPlanThreads - 1) / kPlanThreads : 0;
+    L.blocks = grid_blocks(P, kPlanThreads);
     size_t o = 0;
     L.ctrl = o;   o = align_up(o + 64, 256);                          // [0] ticket, [4..7] KO, KC, S, KS
-    L.status = o; o = align_up(o + (size_t)4 * (L.blocks + 1) * 8, 256);   // one look-back word per counter per block
+    L.status = o; o = align_up(o + (size_t)4 * L.blocks * 8, 256);    // one look-back word per counter per block
     L.rec = o;    o = align_up(o + (size_t)(P > 0 ? P : 1) * 16, 256);
     L.total = o;
     return L;
@@ -72,11 +72,9 @@ struct PlanParams {
 
 __global__ void __launch_bounds__(kPlanThreads) densify_plan_kernel(const __grid_constant__ PlanParams p) {
     __shared__ unsigned long long s_warp[kPlanThreads / 32];
-    __shared__ uint32_t s_bid, s_excl[4];
+    __shared__ uint32_t s_excl[4];
     const int tid = threadIdx.x;
-    if (tid == 0) s_bid = atomicAdd(&p.ctrl[0], 1u);   // ticket: blocks look back only at blocks already running
-    __syncthreads();
-    const uint32_t bid = s_bid;
+    const uint32_t bid = block_ticket(&p.ctrl[0]);
     const int i = (int)(bid * kPlanThreads) + tid;
 
     bool keep_orig = false, keep_clone = false, split = false, keep_split = false;
@@ -256,16 +254,13 @@ int surfel_densify_plan(int P, const float* xyz_gradient_accum, const float* den
                         size_t workspace_bytes, int32_t* totals, void* stream) {
     if (P < 0) { surfel_set_error("surfel_densify_plan: P < 0"); return 1; }
     if (P > kDensifyMaxP) { surfel_set_error("surfel_densify_plan: P = %d exceeds %d", P, kDensifyMaxP); return 1; }
-    if (!workspace || !totals) { surfel_set_error("surfel_densify_plan: NULL workspace or totals"); return 1; }
+    if (!totals) { surfel_set_error("surfel_densify_plan: NULL totals"); return 1; }
     if (P > 0 && (!xyz_gradient_accum || !denom || !scaling || !opacity)) {
         surfel_set_error("surfel_densify_plan: NULL input pointer");
         return 1;
     }
     const DensifyLayout L = densify_layout(P);
-    if (workspace_bytes < L.total) {
-        surfel_set_error("surfel_densify_plan: workspace of %zu bytes, %zu needed", workspace_bytes, L.total);
-        return 1;
-    }
+    if (!workspace_ok("surfel_densify_plan", workspace, workspace_bytes, L.total)) return 1;
     cudaStream_t st = (cudaStream_t)stream;
     char* w = (char*)workspace;
     uint32_t* ctrl = (uint32_t*)(w + L.ctrl);
@@ -274,7 +269,7 @@ int surfel_densify_plan(int P, const float* xyz_gradient_accum, const float* den
         SURFEL_CUDA_OK(cudaMemsetAsync(totals, 0, 4 * sizeof(int32_t), st));
         return 0;
     }
-    SURFEL_CUDA_OK(cudaMemsetAsync(w + L.status, 0, (size_t)4 * (L.blocks + 1) * 8, st));
+    SURFEL_CUDA_OK(cudaMemsetAsync(w + L.status, 0, (size_t)4 * L.blocks * 8, st));
     PlanParams p;
     p.P = P;
     p.accum = xyz_gradient_accum; p.denom = denom; p.scaling = scaling; p.opacity = opacity;
@@ -306,13 +301,10 @@ int surfel_densify_apply(int P, int P_out, int n_split, int n_groups, const surf
         surfel_set_error("surfel_densify_apply: n_groups %d outside [1, %d]", n_groups, SURFEL_DENSIFY_MAX_GROUPS);
         return 1;
     }
-    if (!groups || !workspace) { surfel_set_error("surfel_densify_apply: NULL groups or workspace"); return 1; }
+    if (!groups) { surfel_set_error("surfel_densify_apply: NULL groups"); return 1; }
     if (n_split > 0 && !z) { surfel_set_error("surfel_densify_apply: NULL z with %d split rows", n_split); return 1; }
     const DensifyLayout L = densify_layout(P);
-    if (workspace_bytes < L.total) {
-        surfel_set_error("surfel_densify_apply: workspace of %zu bytes, %zu needed", workspace_bytes, L.total);
-        return 1;
-    }
+    if (!workspace_ok("surfel_densify_apply", workspace, workspace_bytes, L.total)) return 1;
     ApplyTable t;
     t.n = 0; t.P = P; t.rot = t.scale = -1;
     int xyz = -1;

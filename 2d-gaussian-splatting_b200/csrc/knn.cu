@@ -341,12 +341,9 @@ int surfel_knn_mean_sq_dist(int P, const float* xyz, float* out, void* workspace
     if (P < 0) { surfel_set_error("surfel_knn_mean_sq_dist: P < 0"); return 1; }
     if (P > kKnnMaxP) { surfel_set_error("surfel_knn_mean_sq_dist: P = %d exceeds %d", P, kKnnMaxP); return 1; }
     if (P == 0) return 0;
-    if (!xyz || !out || !workspace) { surfel_set_error("surfel_knn_mean_sq_dist: NULL pointer"); return 1; }
+    if (!xyz || !out) { surfel_set_error("surfel_knn_mean_sq_dist: NULL pointer"); return 1; }
     const KnnLayout L = knn_layout(P);
-    if (workspace_bytes < L.total) {
-        surfel_set_error("surfel_knn_mean_sq_dist: workspace of %zu bytes, %zu needed", workspace_bytes, L.total);
-        return 1;
-    }
+    if (!workspace_ok("surfel_knn_mean_sq_dist", workspace, workspace_bytes, L.total)) return 1;
     cudaStream_t st = (cudaStream_t)stream;
     char* w = (char*)workspace;
     uint32_t* ctrl = (uint32_t*)(w + L.ctrl);

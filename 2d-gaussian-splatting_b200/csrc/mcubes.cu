@@ -115,10 +115,8 @@ struct McCtrl {
 
 __global__ void __launch_bounds__(kMcThreads) mc_count_kernel(const __grid_constant__ McCrop c, McCtrl w,
                                                               long long* totals) {
-    __shared__ uint32_t s_warp[kMcThreads / 32], s_bid, s_excl[2];
-    if (threadIdx.x == 0) s_bid = atomicAdd(&w.ctrl[0], 1u);   // ticket: look back only at blocks already running
-    __syncthreads();
-    const uint32_t bid = s_bid;
+    __shared__ uint32_t s_warp[kMcThreads / 32], s_excl[2];
+    const uint32_t bid = block_ticket(&w.ctrl[0]);
     const long long n = (long long)c.s * c.s * c.s;
     const long long i = (long long)bid * kMcThreads + threadIdx.x;
     uint32_t mine = 0;
@@ -202,21 +200,16 @@ __global__ void __launch_bounds__(kMcThreads) mc_unique_kernel(long long n, cons
                                                                float cx, float cy, float cz,
                                                                unsigned long long* __restrict__ ukeys,
                                                                float* __restrict__ verts, long long* n_verts) {
-    __shared__ uint32_t s_warp[kMcThreads / 32], s_bid, s_excl[1];
-    if (threadIdx.x == 0) s_bid = atomicAdd(&w.ctrl[0], 1u);
-    __syncthreads();
-    const uint32_t bid = s_bid;
+    const uint32_t bid = block_ticket(&w.ctrl[0]);
     const long long i = (long long)bid * kMcThreads + threadIdx.x;
     const bool first = i < n && (i == 0 || keys[i] != keys[i - 1]);
-    uint32_t total;
-    const uint32_t excl = block_exclusive_scan<kMcThreads>(first ? 1u : 0u, s_warp, total);
-    block_lookback<1>(w.status, gridDim.x, bid, &total, s_excl);
-    if (bid == gridDim.x - 1 && threadIdx.x == 0) {
-        w.ctrl[1] = s_excl[0] + total;
-        *n_verts = (long long)s_excl[0] + total;
+    const GridScan s = grid_exclusive_scan<kMcThreads>(first ? 1u : 0u, bid, w.status);
+    if (s.last && threadIdx.x == 0) {
+        w.ctrl[1] = s.base + s.total;
+        *n_verts = (long long)s.base + s.total;
     }
     if (!first) return;
-    const long long r = (long long)s_excl[0] + excl;
+    const long long r = s.rank;
     const uint32_t src = vals[i];
     float X = pos[3 * (size_t)src], Y = pos[3 * (size_t)src + 1], Z = pos[3 * (size_t)src + 2];
     inv_contraction(contraction_norm(X, Y, Z), X, Y, Z, radius, cx, cy, cz);
@@ -244,13 +237,12 @@ __global__ void mc_faces_kernel(long long n, const unsigned long long* __restric
 
 struct CropLayout {
     size_t ctrl, status, prefix, total;
-    int blocks;
+    unsigned blocks;
 };
 
 CropLayout crop_layout(int side) {
     CropLayout L;
-    const long long n = (long long)side * side * side;
-    L.blocks = (int)((n + kMcThreads - 1) / kMcThreads);
+    L.blocks = grid_blocks((long long)side * side * side, kMcThreads);
     size_t o = 0;
     L.ctrl = o;   o = align_up(o + 64, 256);
     L.status = o; o = align_up(o + (size_t)2 * L.blocks * 8, 256);
@@ -261,13 +253,13 @@ CropLayout crop_layout(int side) {
 
 struct MergeLayout {
     size_t ctrl, status, sort, ukeys, total;
-    int blocks;
+    unsigned blocks;
 };
 
 MergeLayout merge_layout(long long n) {
     MergeLayout L;
     const size_t m = n > 0 ? (size_t)n : 1;
-    L.blocks = (int)((m + kMcThreads - 1) / kMcThreads);
+    L.blocks = grid_blocks(n, kMcThreads);
     size_t o = 0;
     L.ctrl = o;   o = align_up(o + 64, 256);
     L.status = o; o = align_up(o + (size_t)L.blocks * 8, 256);
@@ -320,12 +312,9 @@ int surfel_mcubes_crop_count(int side, const float* volume, const int* crop, int
                              size_t workspace_bytes, long long* totals, void* stream) {
     McCrop c;
     if (!make_crop("surfel_mcubes_crop_count", side, volume, crop, crops_per_axis, c)) return 1;
-    if (!workspace || !totals) { surfel_set_error("surfel_mcubes_crop_count: NULL workspace or totals"); return 1; }
+    if (!totals) { surfel_set_error("surfel_mcubes_crop_count: NULL totals"); return 1; }
     const CropLayout L = crop_layout(side);
-    if (workspace_bytes < L.total) {
-        surfel_set_error("surfel_mcubes_crop_count: workspace of %zu bytes, %zu needed", workspace_bytes, L.total);
-        return 1;
-    }
+    if (!workspace_ok("surfel_mcubes_crop_count", workspace, workspace_bytes, L.total)) return 1;
     cudaStream_t st = (cudaStream_t)stream;
     char* w = (char*)workspace;
     SURFEL_CUDA_OK(cudaMemsetAsync(w + L.ctrl, 0, 64, st));
@@ -343,17 +332,14 @@ int surfel_mcubes_crop_emit(int side, const float* volume, const double* bounds,
                             void* stream) {
     McCrop c;
     if (!make_crop("surfel_mcubes_crop_emit", side, volume, crop, crops_per_axis, c)) return 1;
-    if (!bounds || !workspace) { surfel_set_error("surfel_mcubes_crop_emit: NULL bounds or workspace"); return 1; }
+    if (!bounds) { surfel_set_error("surfel_mcubes_crop_emit: NULL bounds"); return 1; }
     if (n_records < 0 || n_tris < 0) { surfel_set_error("surfel_mcubes_crop_emit: negative count"); return 1; }
     if ((n_records > 0 && (!vert_keys || !vert_pos)) || (n_tris > 0 && !tri_keys)) {
         surfel_set_error("surfel_mcubes_crop_emit: NULL output");
         return 1;
     }
     const CropLayout L = crop_layout(side);
-    if (workspace_bytes < L.total) {
-        surfel_set_error("surfel_mcubes_crop_emit: workspace of %zu bytes, %zu needed", workspace_bytes, L.total);
-        return 1;
-    }
+    if (!workspace_ok("surfel_mcubes_crop_emit", workspace, workspace_bytes, L.total)) return 1;
     if (n_records == 0 && n_tris == 0) return 0;
     for (int d = 0; d < 3; d++) c.ax[d] = make_lin_axis(bounds[2 * d], bounds[2 * d + 1], side);
     cudaStream_t st = (cudaStream_t)stream;
@@ -384,19 +370,13 @@ int surfel_mcubes_merge(long long n_records, const unsigned long long* vert_keys
     }
     if (n_tris > (1ll << 40)) { surfel_set_error("surfel_mcubes_merge: %lld triangles", n_tris); return 1; }
     if (key_bits < 1 || key_bits > 64) { surfel_set_error("surfel_mcubes_merge: key_bits %d", key_bits); return 1; }
-    if (!center || !workspace || !n_verts) {
-        surfel_set_error("surfel_mcubes_merge: NULL center, workspace or vertex count");
-        return 1;
-    }
+    if (!center || !n_verts) { surfel_set_error("surfel_mcubes_merge: NULL center or vertex count"); return 1; }
     if ((n_records > 0 && (!vert_keys || !vert_pos || !verts)) || (n_tris > 0 && (!tri_keys || !faces))) {
         surfel_set_error("surfel_mcubes_merge: NULL input or output");
         return 1;
     }
     const MergeLayout L = merge_layout(n_records);
-    if (workspace_bytes < L.total) {
-        surfel_set_error("surfel_mcubes_merge: workspace of %zu bytes, %zu needed", workspace_bytes, L.total);
-        return 1;
-    }
+    if (!workspace_ok("surfel_mcubes_merge", workspace, workspace_bytes, L.total)) return 1;
     cudaStream_t st = (cudaStream_t)stream;
     char* w = (char*)workspace;
     SURFEL_CUDA_OK(cudaMemsetAsync(w + L.ctrl, 0, 64, st));

@@ -121,10 +121,7 @@ __global__ void __launch_bounds__(kMpThreads) mp_compress_kernel(long long F, ui
 __global__ void __launch_bounds__(kMpThreads) mp_roots_kernel(long long F, uint32_t* parent, uint32_t* __restrict__ rank,
                                                               uint32_t* ctrl, unsigned long long* status,
                                                               long long* info) {
-    __shared__ uint32_t s_warp[kMpThreads / 32], s_bid, s_excl[1];
-    if (threadIdx.x == 0) s_bid = atomicAdd(&ctrl[0], 1u);
-    __syncthreads();
-    const uint32_t bid = s_bid;
+    const uint32_t bid = block_ticket(&ctrl[0]);
     const long long t = (long long)bid * kMpThreads + threadIdx.x;
     bool root = false;
     if (t < F) {
@@ -132,12 +129,10 @@ __global__ void __launch_bounds__(kMpThreads) mp_roots_kernel(long long F, uint3
         st_parent(parent + t, r);
         root = r == (uint32_t)t;
     }
-    uint32_t total;
-    const uint32_t excl = block_exclusive_scan<kMpThreads>(root ? 1u : 0u, s_warp, total);
-    block_lookback<1>(status, gridDim.x, bid, &total, s_excl);
-    if (root) rank[t] = s_excl[0] + excl;
-    if (bid == gridDim.x - 1 && threadIdx.x == 0) {
-        info[0] = (long long)s_excl[0] + total;
+    const GridScan s = grid_exclusive_scan<kMpThreads>(root ? 1u : 0u, bid, status);
+    if (root) rank[t] = s.rank;
+    if (s.last && threadIdx.x == 0) {
+        info[0] = (long long)s.base + s.total;
         info[1] = ctrl[4];
     }
 }
@@ -183,21 +178,15 @@ __global__ void __launch_bounds__(kMpThreads) mp_mark_kernel(long long F, long l
 __global__ void __launch_bounds__(kMpThreads) mp_vscan_kernel(long long M, uint32_t* vnew, long long* __restrict__ vert_map,
                                                               uint32_t* ctrl, unsigned long long* status,
                                                               long long* info) {
-    __shared__ uint32_t s_warp[kMpThreads / 32], s_bid, s_excl[1];
-    if (threadIdx.x == 0) s_bid = atomicAdd(&ctrl[1], 1u);
-    __syncthreads();
-    const uint32_t bid = s_bid;
+    const uint32_t bid = block_ticket(&ctrl[1]);
     const long long v = (long long)bid * kMpThreads + threadIdx.x;
     const bool marked = v < M && vnew[v] != 0;
-    uint32_t total;
-    const uint32_t excl = block_exclusive_scan<kMpThreads>(marked ? 1u : 0u, s_warp, total);
-    block_lookback<1>(status, gridDim.x, bid, &total, s_excl);
+    const GridScan s = grid_exclusive_scan<kMpThreads>(marked ? 1u : 0u, bid, status);
     if (marked) {
-        const uint32_t r = s_excl[0] + excl;
-        vnew[v] = r;
-        vert_map[r] = v;
+        vnew[v] = s.rank;
+        vert_map[s.rank] = v;
     }
-    if (bid == gridDim.x - 1 && threadIdx.x == 0) info[0] = (long long)s_excl[0] + total;
+    if (s.last && threadIdx.x == 0) info[0] = (long long)s.base + s.total;
 }
 
 __global__ void __launch_bounds__(kMpThreads) mp_fscan_kernel(long long F, long long M, const long long* __restrict__ faces,
@@ -206,10 +195,7 @@ __global__ void __launch_bounds__(kMpThreads) mp_fscan_kernel(long long F, long 
                                                               const uint64_t* kth, const uint32_t* __restrict__ vnew,
                                                               long long* __restrict__ out_faces, uint32_t* ctrl,
                                                               unsigned long long* status, long long* info) {
-    __shared__ uint32_t s_warp[kMpThreads / 32], s_bid, s_excl[1];
-    if (threadIdx.x == 0) s_bid = atomicAdd(&ctrl[2], 1u);
-    __syncthreads();
-    const uint32_t bid = s_bid;
+    const uint32_t bid = block_ticket(&ctrl[2]);
     const long long f = (long long)bid * kMpThreads + threadIdx.x;
     long long v[3] = {0, 0, 0};
     bool keep = false;
@@ -222,18 +208,13 @@ __global__ void __launch_bounds__(kMpThreads) mp_fscan_kernel(long long F, long 
         }
         keep &= v[0] != v[1] && v[1] != v[2] && v[0] != v[2];
     }
-    uint32_t total;
-    const uint32_t excl = block_exclusive_scan<kMpThreads>(keep ? 1u : 0u, s_warp, total);
-    block_lookback<1>(status, gridDim.x, bid, &total, s_excl);
+    const GridScan s = grid_exclusive_scan<kMpThreads>(keep ? 1u : 0u, bid, status);
     if (keep) {
-        const long long r = (long long)s_excl[0] + excl;
 #pragma unroll
-        for (int j = 0; j < 3; j++) out_faces[3 * r + j] = vnew[v[j]];
+        for (int j = 0; j < 3; j++) out_faces[3 * (long long)s.rank + j] = vnew[v[j]];
     }
-    if (bid == gridDim.x - 1 && threadIdx.x == 0) info[1] = (long long)s_excl[0] + total;
+    if (s.last && threadIdx.x == 0) info[1] = (long long)s.base + s.total;
 }
-
-int blocks_of(long long n) { return (int)std::max<long long>(1, (n + kMpThreads - 1) / kMpThreads); }
 
 struct MpLayout {
     size_t ctrl, status_f, status_m, status_c, sort, parent, rank, vnew, total;
@@ -245,9 +226,9 @@ MpLayout mp_layout(long long M, long long F) {
     const size_t f = (size_t)std::max<long long>(F, 1), m = (size_t)std::max<long long>(M, 1), r = 3 * f;
     size_t o = 0;
     L.ctrl = o;     o = align_up(o + 64, 256);
-    L.status_f = o; o = align_up(o + (size_t)blocks_of(F) * 8, 256);
-    L.status_m = o; o = align_up(o + (size_t)blocks_of(M) * 8, 256);
-    L.status_c = o; o = align_up(o + (size_t)blocks_of(F) * 8, 256);
+    L.status_f = o; o = align_up(o + (size_t)grid_blocks(F, kMpThreads) * 8, 256);
+    L.status_m = o; o = align_up(o + (size_t)grid_blocks(M, kMpThreads) * 8, 256);
+    L.status_c = o; o = align_up(o + (size_t)grid_blocks(F, kMpThreads) * 8, 256);
     L.sort = o;     o = align_up(o + radix_sort_workspace_bytes(r), 256);
     L.parent = o;   o = align_up(o + f * 4, 256);
     L.rank = o;     o = align_up(o + f * 4, 256);
@@ -264,15 +245,6 @@ bool sizes_ok(const char* who, long long M, long long F) {
     }
     if (F > kMpMaxFaces) {
         surfel_set_error("%s: %lld faces give %lld edge records; the radix sort takes fewer than 2^30", who, F, 3 * F);
-        return false;
-    }
-    return true;
-}
-
-bool workspace_ok(const char* who, const void* ws, size_t bytes, const MpLayout& L) {
-    if (!ws) { surfel_set_error("%s: NULL workspace", who); return false; }
-    if (bytes < L.total) {
-        surfel_set_error("%s: workspace of %zu bytes, %zu needed", who, bytes, L.total);
         return false;
     }
     return true;
@@ -300,7 +272,7 @@ int surfel_meshpost_clusters(long long n_verts, long long n_faces, const long lo
         return 1;
     }
     const MpLayout L = mp_layout(n_verts, n_faces);
-    if (!workspace_ok(who, workspace, workspace_bytes, L)) return 1;
+    if (!workspace_ok(who, workspace, workspace_bytes, L.total)) return 1;
     cudaStream_t st = (cudaStream_t)stream;
     if (n_faces == 0) {
         SURFEL_CUDA_OK(cudaMemsetAsync(info, 0, 2 * sizeof(long long), st));
@@ -312,35 +284,37 @@ int surfel_meshpost_clusters(long long n_verts, long long n_faces, const long lo
     const RadixSortWs sort = radix_sort_ws(w + L.sort, 3 * (size_t)n_faces, radix_key_bits(M > 0 ? M * M - 1 : 0));
     uint32_t *parent = (uint32_t*)(w + L.parent), *rank = (uint32_t*)(w + L.rank);
     SURFEL_CUDA_OK(cudaMemsetAsync(ctrl, 0, 64, st));
-    SURFEL_CUDA_OK(cudaMemsetAsync(w + L.status_f, 0, (size_t)blocks_of(n_faces) * 8, st));
+    const unsigned nb_f = grid_blocks(n_faces, kMpThreads);
+    SURFEL_CUDA_OK(cudaMemsetAsync(w + L.status_f, 0, (size_t)nb_f * 8, st));
     SURFEL_CUDA_OK(cudaMemsetAsync(cluster_count, 0, (size_t)n_faces * sizeof(int), st));
     const long long n_rec = 3 * n_faces;
     {
         LaunchScope scope(kStMeshpostEdges, st);
-        mp_edges_kernel<<<blocks_of(n_faces), kMpThreads, 0, st>>>(n_faces, n_verts, faces, sort.in.keys, sort.in.vals,
-                                                                   parent, ctrl + 4);
+        mp_edges_kernel<<<nb_f, kMpThreads, 0, st>>>(n_faces, n_verts, faces, sort.in.keys, sort.in.vals, parent,
+                                                     ctrl + 4);
         SURFEL_CUDA_OK(cudaGetLastError());
     }
     if (launch_radix_sort_pairs(sort, (size_t)n_rec, st)) return 1;
     {
         LaunchScope scope(kStMeshpostUnion, st);
-        mp_union_kernel<<<blocks_of(n_rec - 1), kMpThreads, 0, st>>>(n_rec, sort.out.keys, sort.out.vals, parent);
+        mp_union_kernel<<<grid_blocks(n_rec - 1, kMpThreads), kMpThreads, 0, st>>>(n_rec, sort.out.keys, sort.out.vals,
+                                                                                    parent);
         SURFEL_CUDA_OK(cudaGetLastError());
     }
     {
         LaunchScope scope(kStMeshpostUnion, st);
-        mp_compress_kernel<<<blocks_of(n_faces), kMpThreads, 0, st>>>(n_faces, parent);
+        mp_compress_kernel<<<nb_f, kMpThreads, 0, st>>>(n_faces, parent);
         SURFEL_CUDA_OK(cudaGetLastError());
     }
     {
         LaunchScope scope(kStMeshpostLabel, st);
-        mp_roots_kernel<<<blocks_of(n_faces), kMpThreads, 0, st>>>(n_faces, parent, rank, ctrl,
-                                                                   (unsigned long long*)(w + L.status_f), info);
+        mp_roots_kernel<<<nb_f, kMpThreads, 0, st>>>(n_faces, parent, rank, ctrl,
+                                                     (unsigned long long*)(w + L.status_f), info);
         SURFEL_CUDA_OK(cudaGetLastError());
     }
     {
         LaunchScope scope(kStMeshpostLabel, st);
-        mp_label_kernel<<<blocks_of(n_faces), kMpThreads, 0, st>>>(n_faces, parent, rank, face_cluster, cluster_count);
+        mp_label_kernel<<<nb_f, kMpThreads, 0, st>>>(n_faces, parent, rank, face_cluster, cluster_count);
         SURFEL_CUDA_OK(cudaGetLastError());
     }
     return 0;
@@ -365,41 +339,40 @@ int surfel_meshpost_compact(long long n_verts, long long n_faces, const long lon
         return 1;
     }
     const MpLayout L = mp_layout(n_verts, n_faces);
-    if (!workspace_ok(who, workspace, workspace_bytes, L)) return 1;
+    if (!workspace_ok(who, workspace, workspace_bytes, L.total)) return 1;
     cudaStream_t st = (cudaStream_t)stream;
     char* w = (char*)workspace;
     uint32_t* ctrl = (uint32_t*)(w + L.ctrl);
     const RadixSortWs sort = radix_sort_ws(w + L.sort, 3 * (size_t)n_faces, radix_key_bits((unsigned long long)n_faces));
     uint32_t* vnew = (uint32_t*)(w + L.vnew);
     SURFEL_CUDA_OK(cudaMemsetAsync(ctrl, 0, 64, st));
-    SURFEL_CUDA_OK(cudaMemsetAsync(w + L.status_m, 0, (size_t)blocks_of(n_verts) * 8, st));
-    SURFEL_CUDA_OK(cudaMemsetAsync(w + L.status_c, 0, (size_t)blocks_of(n_faces) * 8, st));
+    const unsigned nb_m = grid_blocks(n_verts, kMpThreads), nb_f = grid_blocks(n_faces, kMpThreads);
+    SURFEL_CUDA_OK(cudaMemsetAsync(w + L.status_m, 0, (size_t)nb_m * 8, st));
+    SURFEL_CUDA_OK(cudaMemsetAsync(w + L.status_c, 0, (size_t)nb_f * 8, st));
     SURFEL_CUDA_OK(cudaMemsetAsync(vnew, 0, (size_t)std::max<long long>(n_verts, 1) * 4, st));
     {
         LaunchScope scope(kStMeshpostCompact, st);
-        mp_count_keys_kernel<<<blocks_of(n_clusters), kMpThreads, 0, st>>>(n_clusters, cluster_count, sort.in.keys,
-                                                                            sort.in.vals);
+        mp_count_keys_kernel<<<grid_blocks(n_clusters, kMpThreads), kMpThreads, 0, st>>>(n_clusters, cluster_count,
+                                                                                          sort.in.keys, sort.in.vals);
         SURFEL_CUDA_OK(cudaGetLastError());
     }
     if (launch_radix_sort_pairs(sort, (size_t)n_clusters, st)) return 1;
     const uint64_t* kth = sort.out.keys + index;
     {
         LaunchScope scope(kStMeshpostCompact, st);
-        mp_mark_kernel<<<blocks_of(n_faces), kMpThreads, 0, st>>>(n_faces, n_verts, faces, face_cluster, cluster_count,
-                                                                  kth, vnew);
+        mp_mark_kernel<<<nb_f, kMpThreads, 0, st>>>(n_faces, n_verts, faces, face_cluster, cluster_count, kth, vnew);
         SURFEL_CUDA_OK(cudaGetLastError());
     }
     {
         LaunchScope scope(kStMeshpostCompact, st);
-        mp_vscan_kernel<<<blocks_of(n_verts), kMpThreads, 0, st>>>(n_verts, vnew, vert_map, ctrl,
-                                                                   (unsigned long long*)(w + L.status_m), info);
+        mp_vscan_kernel<<<nb_m, kMpThreads, 0, st>>>(n_verts, vnew, vert_map, ctrl,
+                                                     (unsigned long long*)(w + L.status_m), info);
         SURFEL_CUDA_OK(cudaGetLastError());
     }
     {
         LaunchScope scope(kStMeshpostCompact, st);
-        mp_fscan_kernel<<<blocks_of(n_faces), kMpThreads, 0, st>>>(n_faces, n_verts, faces, face_cluster, cluster_count,
-                                                                   kth, vnew, out_faces, ctrl,
-                                                                   (unsigned long long*)(w + L.status_c), info);
+        mp_fscan_kernel<<<nb_f, kMpThreads, 0, st>>>(n_faces, n_verts, faces, face_cluster, cluster_count, kth, vnew,
+                                                     out_faces, ctrl, (unsigned long long*)(w + L.status_c), info);
         SURFEL_CUDA_OK(cudaGetLastError());
     }
     return 0;

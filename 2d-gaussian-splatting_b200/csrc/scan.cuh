@@ -1,15 +1,17 @@
 // scan.cuh — the single-pass decoupled look-back scan that chains a count across a whole grid in one launch, shared
-// by preprocess_fwd.cu (tile offsets and R), densify.cu (the plan's four counters) and mcubes.cu (count and merge).
+// by preprocess_fwd.cu (tile offsets and R), densify.cu (the plan's four counters), mcubes.cu (count and merge),
+// meshpost.cu, chamfer.cu and cull.cu.  grid_exclusive_scan is the whole protocol for one count per thread; kernels
+// that scan several counters, or (preprocess) publish early and look back late, call the parts it is built from.
 //
 // Each block owns one 64-bit status word per counter: bits 0-31 hold a count, bit 32 (kFlagAgg) marks it as the
 // block's own aggregate and bit 33 (kFlagPrefix) as the inclusive prefix of every block up to and including it; a
 // word of 0 is not yet published.  A block publishes its aggregate (block 0 its prefix) as soon as it has it, then
 // one warp walks back 32 predecessors at a time, summing aggregates until it meets a prefix, and publishes its own
 // inclusive prefix.  The protocol holds only under these conditions:
-//  * the status words are zeroed before the launch (the callers' cudaMemsetAsync);
-//  * block indices come from a ticket (an atomicAdd on a zeroed counter by the block's first thread), not from
-//    blockIdx: a block then waits only on blocks that have already started, so the spin always ends, whatever
-//    order the hardware schedules blocks in;
+//  * the grid has one status word per counter per block (grid_blocks sizes both), and the status words and the
+//    ticket word are zeroed before the launch (the callers' cudaMemsetAsync);
+//  * block indices come from a ticket (block_ticket), not from blockIdx: a block then waits only on blocks that have
+//    already started, so the spin always ends, whatever order the hardware schedules blocks in;
 //  * relaxed loads and stores suffice because the count travels in the same 64-bit word as its flag: a reader
 //    that sees the flag sees the count, and no other data is passed from block to block;
 //  * a count, and so the grid-wide total, must fit the 32-bit field.
@@ -20,6 +22,19 @@
 namespace surfel {
 
 constexpr unsigned long long kFlagAgg = 1ull << 32, kFlagPrefix = 2ull << 32;
+
+// Blocks of `threads` that cover n items, at least one (a scan over nothing still has a block to write its zero
+// total): the grid of a scan and the number of its status words per counter.
+inline unsigned grid_blocks(long long n, int threads) { return n > 0 ? (unsigned)((n + threads - 1) / threads) : 1u; }
+
+// The block's index in ticket order: thread 0 draws it from the zeroed word `ticket`, and every thread of the block
+// calls this and gets it.
+__device__ __forceinline__ uint32_t block_ticket(uint32_t* ticket) {
+    __shared__ uint32_t s_bid;
+    if (threadIdx.x == 0) s_bid = atomicAdd(ticket, 1u);
+    __syncthreads();
+    return s_bid;
+}
 
 __device__ __forceinline__ unsigned long long ld_status(const unsigned long long* p) {
     unsigned long long v;
@@ -104,6 +119,24 @@ __device__ __forceinline__ void block_lookback(unsigned long long* status, int n
         if ((tid & 31) == 0) s_excl[warp] = excl;
     }
     __syncthreads();
+}
+
+struct GridScan {
+    uint32_t rank;    // the thread's exclusive prefix over the whole grid
+    uint32_t base;    // the sum over the blocks before this one
+    uint32_t total;   // this block's sum
+    bool last;        // this is the grid's last block, whose base + total is the grid's total
+};
+
+// Grid-wide exclusive scan of one count per thread over kThreads-thread blocks, block `bid` from block_ticket and
+// status the grid's gridDim.x zeroed words.  Every thread of the block calls it.
+template <int kThreads>
+__device__ __forceinline__ GridScan grid_exclusive_scan(uint32_t mine, uint32_t bid, unsigned long long* status) {
+    __shared__ uint32_t s_warp[kThreads / 32], s_excl[1];
+    uint32_t total;
+    const uint32_t excl = block_exclusive_scan<kThreads>(mine, s_warp, total);
+    block_lookback<1>(status, gridDim.x, bid, &total, s_excl);
+    return GridScan{s_excl[0] + excl, s_excl[0], total, bid == gridDim.x - 1};
 }
 
 }  // namespace surfel
